@@ -4,8 +4,8 @@
         --ep 8 --zero 1 --batch_size 1 --max_length 4096 --steps 100 --save_dir ckpt --save_interval 50
     torchrun --nproc-per-node 2 --master-addr 127.0.0.1 applications/ColossalMoE/train.py --model mixtral-tiny --ep 2 --steps 10
 
-Experts are sharded over the `--ep` group (dropless dispatch, grouped tcgen05 GEMMs, fused NVLink dispatch / combine on a
-B200 node), attention / dense layers over `--tp`, layers over `--pp`; the remaining ranks are data parallel (`--zero`).
+Experts are sharded over the `--ep` group (dropless dispatch, grouped wgmma GEMMs, fused NVLink dispatch / combine on an
+NVSwitch node), attention / dense layers over `--tp`, layers over `--pp`; the remaining ranks are data parallel (`--zero`).
 The loss adds the routers' load-balancing terms; every `--log_interval` steps the expert load share is printed (max share
 x experts: 1.0 = balanced).  `--pretrained` imports a HuggingFace Mixtral / DeepSeek-MoE directory (`models.hf_io`),
 `--load_checkpoint` resumes.  Data: jsonl `{"text": ...}` via `--dataset`, else random tokens.

@@ -4,8 +4,8 @@
 This is the reference's own `BUILD_EXT=1` recipe (`setup.py:72-96`: `ext.build_aot()` for every extension) restricted to
 those two, executed against the UNMODIFIED sources installed in `baseline/_ref`; the built modules land in
 `baseline/_ref/colossalai/_C/` where the reference's `KernelLoader` looks first (`extensions/cpp_extension.py:57-61,130`).
-There is no GPU on the build box, so the arch list is pinned to sm_100 (the cross-compile branch of the reference's
-`set_cuda_arch_list` only knows architectures up to 8.6) and `torch.cuda.get_device_capability` is answered with (10, 0)
+There is no GPU on the build box, so the arch list is pinned to sm_90 (the cross-compile branch of the reference's
+`set_cuda_arch_list` only knows architectures up to 8.6) and `torch.cuda.get_device_capability` is answered with (9, 0)
 for `get_cuda_cc_flag()`.  `-march=native` of the CPU Adam is replaced by an explicit `-march=x86-64-v3` (AVX2) so the
 binary does not depend on the build host's CPU.
 
@@ -26,7 +26,7 @@ def main() -> int:
         print("[build_ref_ext] already built:", sorted(os.listdir(out_dir)))
         return 0
     os.environ.setdefault("FORCE_CUDA", "1")
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 4))
     sys.path[:] = [p for p in sys.path if os.path.abspath(p or ".") != ROOT]
     sys.path.insert(0, REF)
@@ -37,8 +37,8 @@ def main() -> int:
     import torch
 
     if not torch.cuda.is_available():
-        torch.cuda.get_device_capability = lambda *a, **k: (10, 0)     # cross-compiling for the B200 boxes
-        torch.cuda.get_arch_list = lambda: ["sm_100"]
+        torch.cuda.get_device_capability = lambda *a, **k: (9, 0)      # cross-compiling for the H100 boxes
+        torch.cuda.get_arch_list = lambda: ["sm_90"]
     from setuptools import setup
     from torch.utils.cpp_extension import BuildExtension
 

@@ -123,7 +123,7 @@ def _unavailable(why: str) -> None:
 
 def run_reference_arm(args) -> None:
     if not os.path.isdir(os.path.join(REF, "colossalai")):
-        _unavailable("baseline/_ref is missing (pip install --no-deps --target baseline/_ref /root/reference not done)")
+        _unavailable("baseline/_ref is missing (pip install --no-deps --target baseline/_ref <reference checkout> not done)")
         return
     # make sure OUR package is not importable by accident on this path
     sys.path[:] = [p for p in sys.path if os.path.abspath(p or ".") != ROOT]

@@ -1,23 +1,27 @@
 #!/usr/bin/env python
-"""Flagship benchmark: Llama-3-8B training step (fwd + bwd + AdamW), tokens/s over the whole job.
+"""Flagship benchmark: Llama-3 training step (fwd + bwd + AdamW), tokens/s over the whole job.
 
     python bench.py --gpus N --steps K --warmup W                 # our framework (N=1 runs in-process)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W                    # N > 1, one rank per GPU
     python bench.py --impl reference ...                          # the UNMODIFIED reference from baseline/_ref
 
-Metric / config follow BASELINE.json: tokens/sec (whole box, device-timed, max over ranks), Llama-3-8B, bf16,
-synthetic tokens, random-init weights, weak scaling (one 4096-token sequence per GPU per micro-step, 8 micro-steps per
-optimizer step).  Parity: reference `examples/language/llama/benchmark.py`.
+Metric / config: tokens/sec (whole box, device-timed, max over ranks), bf16, synthetic tokens, random-init weights,
+weak scaling (one 4096-token sequence per GPU per micro-step, 8 micro-steps per optimizer step).  Model: Llama-3-8B on
+N > 1 GPUs; on one 80 GB H100 the 8B model's fp32 master weights and AdamW moments alone (~128 GB) do not fit, so N = 1
+defaults to the Llama-3.2-1B shape (`llama3.2-1b`).  Parity: reference `examples/language/llama/benchmark.py`.
+
+`--dump-outputs DIR` writes what the last timed step computed - its loss (`loss.npy`, float64) and a fixed, seeded
+sample of every updated parameter (`params_sample.npy`, float32, <= 64 MB) - so two builds can be compared output for
+output on identical inputs.
 
 Parallelism (`--parallelism`, same flag and same spellings for both arms):
     tp        the configuration BASELINE.json names: TP = N + Megatron sequence parallelism over NVSwitch (`tpN+sp`)
     dp        pure data parallel with ZeRO-1 optimizer-state sharding (`zero1(dpN)`)
     both      (default) the headline `value` is the `tp` row; the `dp` row is measured in the same process with the
-              same timing rules and reported under `rows` - for an 8B model on 180 GB GPUs plain data parallelism
-              scales better than TP=8, and the line says so instead of hiding it.
+              same timing rules and reported under `rows`.
 At N = 1 the two coincide (`tp1`).  `config.parallelism` of the two arms is the same string whenever they ran the same
-thing, so the driver's same-config check compares like with like.
+thing, so a comparison of two runs compares like with like.
 """
 from __future__ import annotations
 
@@ -34,8 +38,6 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 os.environ.setdefault("PYTORCH_CUDA_ALLOC_CONF", "expandable_segments:True")
 
-BASELINE_TOKENS_PER_S_8GPU = 25.83 * 4096      # BASELINE.md B1: 25.83 samples/s x 4096 tokens on 8x B200 (7B)
-
 
 def parse_args():
     p = argparse.ArgumentParser()
@@ -43,7 +45,8 @@ def parse_args():
     p.add_argument("--steps", type=int, default=5)
     p.add_argument("--warmup", type=int, default=3)
     p.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    p.add_argument("--model", default=os.environ.get("CB200_BENCH_MODEL", "llama3-8b"))
+    p.add_argument("--model", default=os.environ.get("CB200_BENCH_MODEL", ""),
+                   help="model preset (default: llama3-8b on N > 1 GPUs, llama3.2-1b on one GPU)")
     p.add_argument("--seq", type=int, default=4096)
     p.add_argument("--mbs", type=int, default=1, help="sequences per GPU per step (weak scaling)")
     p.add_argument("--accum", type=int, default=int(os.environ.get("CB200_BENCH_ACCUM", "8")),
@@ -60,11 +63,16 @@ def parse_args():
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--profile", default="", help="after the timed region, run ONE extra step under torch.profiler on "
                                                  "rank 0 and write the per-kernel table to this path")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", default="", metavar="DIR",
+                   help="after the timed steps, write the last step's loss and a seeded parameter sample as .npy to DIR")
+    args = p.parse_args()
+    if not args.model:
+        args.model = "llama3-8b" if args.gpus > 1 else "llama3.2-1b"
+    return args
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -130,12 +138,12 @@ def _init_dist(args):
     return torch.distributed.get_rank(), torch.distributed.get_world_size()
 
 
-METRIC = "tokens/sec (whole job, device-timed, max over ranks) Llama-3-8B training step (fwd+bwd+AdamW)"
-L2_NOTE = "working set per step (>= 2 GB weights+activations per layer) >> 126 MB L2; no explicit flush"
+METRIC = "tokens/sec (whole job, device-timed, max over ranks) Llama-3 training step (fwd+bwd+AdamW)"
+L2_NOTE = "working set per step (>= 0.5 GB weights+activations per layer) >> 50 MB L2; no explicit flush"
 
 
 def row_label(kind: str, world: int, tp: int = 0, pp: int = 1, sp_mode: str = "split_gather", zero: int = 0) -> str:
-    """One spelling of a parallel layout for BOTH arms (the driver compares `config.parallelism` across arms)."""
+    """One spelling of a parallel layout for BOTH arms (`config.parallelism` is compared across arms)."""
     if kind == "dp" and world > 1:
         return f"zero1(dp{world})"
     tp = tp or world
@@ -153,7 +161,28 @@ def shared_config(args, world: int, parallelism: str) -> dict:
             "grad_accum": args.accum, "optimizer": "AdamW (fp32 master + moments, grad-norm clip 1.0)", "l2": L2_NOTE}
 
 
-def _measure_ours(args, kind: str, rank: int, world: int, steps: int, with_e2e: bool, profile_path: str = "") -> dict:
+def _dump_outputs(model, loss, out_dir: str, rank: int) -> None:
+    """The last timed step's results as numpy files: the loss and a fixed, seeded sample of the updated parameters."""
+    import numpy as np
+    import torch
+
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    gen = torch.Generator().manual_seed(2024)
+    params = sorted(model.named_parameters(), key=lambda kv: kv[0])
+    per = max(1, (16 << 20) // max(1, len(params)))          # <= 16 M float32 values = 64 MB in all
+    chunks = []
+    for _, p in params:
+        flat = p.detach().reshape(-1)
+        idx = torch.randint(0, flat.numel(), (min(per, flat.numel()),), generator=gen)
+        chunks.append(flat[idx.to(flat.device)].float().cpu())
+    np.save(os.path.join(out_dir, "params_sample.npy"), torch.cat(chunks).numpy().astype(np.float32))
+
+
+def _measure_ours(args, kind: str, rank: int, world: int, steps: int, with_e2e: bool, profile_path: str = "",
+                  dump_dir: str = "") -> dict:
     """Build the model under one parallel layout through the public API (Booster + HybridParallelPlugin), time
     `steps` optimizer steps, tear everything down again."""
     import gc
@@ -267,6 +296,8 @@ def _measure_ours(args, kind: str, rank: int, world: int, steps: int, with_e2e: 
     launches = launch_counter.count
     by_name = dict(launch_counter.by_name)
     clocks = sampler.stop() if rank == 0 else {}
+    if dump_dir:
+        _dump_outputs(model, loss_val, dump_dir, rank)
     e2e = None
     if with_e2e:
         ms_e, wall_e, _ = timed(steps, e2e=True)
@@ -310,22 +341,22 @@ def run_ours(args) -> dict:
         kinds = kinds[:1]                           # tp1 == dp1
     rows = []
     for i, kind in enumerate(kinds):
-        # the headline row runs the K steps the driver asked for; the companion row at least 3 and half of K
-        steps = args.steps if i == 0 else max(3, args.steps // 2)
+        # every row (the headline and the companion layout) times exactly --steps optimizer steps
+        steps = args.steps
         rows.append(_measure_ours(args, kind, rank, world, steps, with_e2e=not args.no_e2e,
-                                  profile_path=args.profile if i == 0 else ""))
+                                  profile_path=args.profile if i == 0 else "",
+                                  dump_dir=args.dump_outputs if i == 0 else ""))
     head = rows[0]
     result = {
         "metric": METRIC, "value": head["value"], "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": head["ms_per_step"], "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": head["value"] / (BASELINE_TOKENS_PER_S_8GPU * world / 8.0), "dtype": "bf16",
+        "dtype": "bf16",
         "data": "synthetic tokens, random-init weights", "impl": "ours",
         "config": shared_config(args, world, head["parallelism"]),
         "detail": {"comm_backend": head["comm_backend"], "grad_ckpt_ratio": args.grad_ckpt,
                    "optimizer_impl": "one-launch multi-tensor AdamW over the flat fp32 master / moment arenas",
                    "attention": os.environ.get("CB200_ATTN_BACKEND", "default"),
-                   "gemm": os.environ.get("CB200_GEMM_BACKEND", "default"),
-                   "baseline_note": "vs_baseline = value / (published 8xB200 7B number scaled to N GPUs)"},
+                   "gemm": os.environ.get("CB200_GEMM_BACKEND", "default")},
         "clocks": head["clocks"], "gpu_launches": head["gpu_launches"], "launches_by_kernel": head["launches_by_kernel"],
         "loss": head["loss"], "peak_mem_mib": head["peak_mem_mib"], "wall_ms_per_step": head["wall_ms_per_step"],
         "tflops_per_gpu": head["tflops_per_gpu"],

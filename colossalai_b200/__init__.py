@@ -1,8 +1,8 @@
-"""colossalai_b200 — a B200-native (sm_100a) hybrid-parallel training & inference framework.
+"""colossalai_b200 — a H100-native (sm_90a) hybrid-parallel training & inference framework.
 
 Capability parity target: hpcaitech/ColossalAI 0.5.0 (see SURVEY.md).  The public surface mirrors the
 reference's (`launch*`, `Booster` + plugins, `ShardFormer`, pipeline schedules, ZeRO / Gemini, inference
-engine) while the compute path is hand-written CUDA for sm_100a (tcgen05/TMEM/TMA) plus fused
+engine) while the compute path is hand-written CUDA for sm_90a (wgmma/TMA) plus fused
 compute+collective kernels over NVLink peer memory; NCCL is the control plane and the multi-node fallback.
 """
 from .initialize import (

@@ -1,5 +1,5 @@
 """Hardware constants the analyzers price things with (reference `_analyzer/envs.py` `MeshConfig`: TFLOPS, bandwidth,
-PCIe).  Defaults are one B200 inside an NVSwitch domain; `from_measured` reads the repo's `MEASURED_PEAKS.json`."""
+PCIe).  Defaults are one GPU inside an NVSwitch domain; `from_measured` reads the repo's `MEASURED_PEAKS.json`."""
 from __future__ import annotations
 
 import json

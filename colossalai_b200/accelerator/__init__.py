@@ -1,5 +1,5 @@
 """Device abstraction.  Parity: reference `colossalai/accelerator/{api,base_accelerator,cuda_accelerator,
-cpu_accelerator}.py`.  Only two targets exist here by design: B200 (`cuda`, NCCL) and the CPU plumbing tier
+cpu_accelerator}.py`.  Only two targets exist here by design: the H100 (`cuda`, NCCL) and the CPU plumbing tier
 (`cpu`, gloo) — no multi-vendor dispatch."""
 from __future__ import annotations
 

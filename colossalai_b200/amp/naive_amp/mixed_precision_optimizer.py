@@ -1,7 +1,7 @@
 """Mixed-precision optimizer: low-precision working params, fp32 master copy + moments.
 
 Parity: reference `colossalai/amp/naive_amp/mixed_precision_optimizer.py:37-224` (master weights, unscale + clip,
-overflow skip, `update_master_params`).  B200-first fast path: when the wrapped optimizer is an Adam-family optimizer
+overflow skip, `update_master_params`).  H100-first fast path: when the wrapped optimizer is an Adam-family optimizer
 of ours and everything is on the GPU, ONE fused kernel launch per param group reads the bf16 grad, applies the
 device-resident unscale x clip coefficient, updates the fp32 master + moments and writes the bf16 working copy —
 no separate unscale pass, no grad fp32 materialisation, no master->working copy pass, no host sync for the norm.

@@ -7,7 +7,7 @@ device budget, and stream them in ahead of use.
   transfer hides under the compute of the layers in between; selection accounts for the hidden part.
 
 `memory_optimize(model, budget)` applies a plan with forward pre/post hooks (fetch / release), pinned host copies and a
-side CUDA stream.  On B200 the host link is PCIe Gen5 / NVLink-C2C class, so the default bandwidth is 50 GB/s.
+side CUDA stream.  The default host-link bandwidth is 50 GB/s (PCIe Gen5 x16 class).
 
 Parity: reference `colossalai/auto_parallel/offload/{solver.py:1-520 (SynGreedySolver, AsynGreedySolver),
 amp_optimizer.py, base_offload_module.py, runtime.py (pre-fwd / post-bwd upload-offload ops), mem_optimize.py:1-60}`.

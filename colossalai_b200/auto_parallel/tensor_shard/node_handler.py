@@ -33,7 +33,7 @@ __all__ = ["HandlerContext", "generate_strategies", "node_shape", "tensor_operan
 class HandlerContext:
     gm: fx.GraphModule
     mesh: DeviceMesh
-    peak_flops: float = 1.4e15          # measured cuBLAS bf16 on B200 (MEASURED_PEAKS.json order of magnitude)
+    peak_flops: float = 1.4e15          # order of magnitude of a dense bf16 tensor-core GPU (H100 SXM data sheet: 0.99e15)
     hbm_bw: float = 6.0e12              # measured copy bandwidth
     shard_inputs: bool = True           # placeholders may be batch-split
     train: bool = True

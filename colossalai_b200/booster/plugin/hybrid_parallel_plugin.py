@@ -3,7 +3,7 @@
 Parity: reference `colossalai/booster/plugin/hybrid_parallel_plugin.py:59-1529` (`HybridParallelModule`,
 `HybridParallel{Naive,AMP,Zero}Optimizer`, `HybridParallelPlugin.__init__/configure/execute_pipeline`, grad-norm
 reduction over tp/pp, tied-embedding / SP-partial / DP gradient syncs, dataloader with DistributedSampler over dp).
-B200 additions: `comm_backend="fused"` routes TP/SP linears through the fused compute+collective kernels; the AMP
+Additions: `comm_backend="fused"` routes TP/SP linears through the fused compute+collective kernels; the AMP
 optimizer runs the single-launch fused Adam (see amp/naive_amp/mixed_precision_optimizer.py).
 """
 from __future__ import annotations
@@ -368,7 +368,7 @@ class HybridParallelNaiveOptimizer(OptimizerWrapper, _HybridNormMixin):
 
 
 class HybridParallelAMPOptimizer(MixedPrecisionOptimizer, _HybridNormMixin):
-    """bf16/fp16 working params + fp32 master (fused single-launch Adam on B200)."""
+    """bf16/fp16 working params + fp32 master (fused single-launch Adam)."""
 
     def __init__(self, optim: Optimizer, model: HybridParallelModule, use_pipeline: bool, param_info: Dict,
                  precision: str = "fp16", initial_scale: float = 2**16, min_scale: float = 1,
@@ -464,7 +464,7 @@ class HybridParallelPlugin(PipelinePluginBase):
         self.tp_size, self.pp_size = tp_size, pp_size
         self.precision, self.zero_stage = precision, zero_stage
         self.cpu_offload = cpu_offload
-        # with cpu_offload: fraction of the optimizer state kept in pinned host memory (tiering between 180 GB HBM and
+        # with cpu_offload: fraction of the optimizer state kept in pinned host memory (tiering between HBM and
         # DRAM that composes with TP x PP - the reference only has Gemini's tiering without PP, or all-or-nothing ZeRO
         # offload: `hybrid_parallel_plugin.py:666-719`)
         self.offload_optim_frac = offload_optim_frac

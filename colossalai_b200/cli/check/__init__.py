@@ -51,7 +51,7 @@ def _run(args: argparse.Namespace, extra) -> int:
     if info["torch CUDA"] and info["system CUDA (nvcc)"] != "N/A":
         same = info["system CUDA (nvcc)"].split(".")[0] == str(info["torch CUDA"]).split(".")[0]
         print(f"CUDA major version match (system vs torch): {'yes' if same else 'NO'}")
-    print("Target architecture: sm_100a (kernels are compiled with -gencode arch=compute_100a,code=sm_100a)")
+    print("Target architecture: sm_90a (kernels are compiled with -gencode arch=compute_90a,code=sm_90a)")
     return 0
 
 

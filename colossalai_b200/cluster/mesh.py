@@ -1,7 +1,7 @@
 """N-D cartesian rank mesh with lazily-created, cached process groups.
 
 Parity: reference `colossalai/cluster/process_group_mesh.py:25-276` (`ProcessGroupMesh`: ravel/unravel,
-`get_group_along_axis`, `create_group_along_axis`, wrap-around neighbours for PP).  The B200-first addition
+`get_group_along_axis`, `create_group_along_axis`, wrap-around neighbours for PP).  The H100-first addition
 is `DeviceMesh`: the same object with *named* axes (dp, pp, ep, sp, tp) so higher layers ask for
 `mesh.group("tp")` and fused kernels can cache symmetric-memory handles per axis group.
 """

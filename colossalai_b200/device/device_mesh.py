@@ -5,7 +5,7 @@ mesh_beta, init_process_group)`, per-axis process groups, `global_rank_to_local_
 formulas).  The runtime mesh of the training stack is `colossalai_b200.cluster.DeviceMesh` (named axes); this class is
 the analysable one: it can exist without any process group and prices collectives.
 
-Default alpha/beta describe a B200 NVSwitch domain: every pair of GPUs sees the same ~1.5 us launch+sync latency and
+Default alpha/beta describe an NVSwitch domain: every pair of GPUs sees the same ~1.5 us launch+sync latency and
 770 GB/s per direction, so a logical axis costs the same wherever it is placed (no ring-per-link penalty).
 """
 from __future__ import annotations

@@ -3,7 +3,7 @@ builds and an availability probe.
 
 Parity: reference `extensions/{base_extension.py:8-82 (_Extension ABC), cpp_extension.py:13-138, cuda_extension.py:18-118,
 __init__.py:13-25 (ALL_EXTENSIONS)}` — there the builds go through `torch.utils.cpp_extension` + pybind; here every
-library is a plain C ABI `.so` compiled by `nvcc -gencode arch=compute_100a,code=sm_100a` (or `g++`) straight into the
+library is a plain C ABI `.so` compiled by `nvcc -gencode arch=compute_90a,code=sm_90a` (or `g++`) straight into the
 source tree and bound with ctypes (`kernel/loader.py`), so the extension objects are thin descriptors over that loader.
 """
 from __future__ import annotations
@@ -42,7 +42,7 @@ class _Extension(ABC):
         return [loader.CSRC / s for s in loader.LIBS[self._lib]["sources"]]
 
     def is_available(self) -> bool:
-        """Sources present and the matching compiler on PATH (nvcc cross-compiles sm_100a without a GPU)."""
+        """Sources present and the matching compiler on PATH (nvcc cross-compiles sm_90a without a GPU)."""
         import shutil
 
         kind = loader.LIBS[self._lib]["kind"]
@@ -64,7 +64,7 @@ class _Extension(ABC):
 
 
 class CudaExtension(_Extension):
-    """sm_100a CUDA library (`-gencode arch=compute_100a,code=sm_100a -lineinfo -O3`)."""
+    """sm_90a CUDA library (`-gencode arch=compute_90a,code=sm_90a -lineinfo -O3`)."""
 
 
 class CppExtension(_Extension):
@@ -76,7 +76,7 @@ def _make(name: str, lib: str) -> _Extension:
     return cls(name, lib)
 
 
-# reference extension names -> our libraries (plus the B200-only ones)
+# reference extension names -> our libraries (plus the ones the reference does not have)
 ALL_EXTENSIONS: Dict[str, _Extension] = {n: _make(n, lib) for n, lib in {
     "cpu_adam_x86": "cb200_cpu_adam",
     "cpu_adam_arm": "cb200_cpu_adam",

@@ -3,7 +3,7 @@
 Parity: reference `colossalai/inference/kv_cache/kvcache_manager.py:18-604`: per-layer K / V tensors of fixed-size
 blocks, free-list allocation for a whole prompt / one decode token / n speculative tokens, block-table maintenance,
 StreamingLLM window eviction, a logical-only RPC variant.
-Layout (B200-first, see kernel/csrc/inference.cu): K and V are both `[num_blocks, block_size, kv_heads, head_dim]`.
+Layout (H100-first, see kernel/csrc/inference.cu): K and V are both `[num_blocks, block_size, kv_heads, head_dim]`.
 """
 from __future__ import annotations
 

@@ -3,7 +3,7 @@ decode (paged split-KV attention over the block tables).
 
 Parity: reference `colossalai/inference/modeling/backends/attention_backend.py:40-170` (`AttentionMetaData`,
 `CudaAttentionBackend`, `TritonAttentionBackend`, `get_attention_backend`).  There is no Triton here: the CUDA backend
-uses the flash varlen kernel for prefill and our sm_100a paged-decode kernel (`kernel/csrc/inference.cu`); the
+uses the flash varlen kernel for prefill and our sm_90a paged-decode kernel (`kernel/csrc/inference.cu`); the
 reference backend is plain PyTorch (CPU tests, numerics oracle).
 """
 from __future__ import annotations

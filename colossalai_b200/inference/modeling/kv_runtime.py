@@ -64,7 +64,7 @@ class PagedKVRuntime:
         return self._attend_full(q, k, v, kc, vc, scale, alibi_slopes)
 
     def _native_prefill(self, q, k, v, scale, window: int, alibi_slopes) -> Optional[torch.Tensor]:
-        """Sliding-window / ALiBi prefill inside the tcgen05 flash kernel (packed batch, device-resident boundaries);
+        """Sliding-window / ALiBi prefill inside the wgmma flash kernel (packed batch, device-resident boundaries);
         None when the tensors are outside the kernel's envelope (CPU tests, head_dim other than 64 / 128, fp32)."""
         from ...ops import flash_attn_native as fan
 

@@ -1,7 +1,7 @@
 """Distributed bring-up.
 
 Parity: reference `colossalai/initialize.py:33-197` (launch / launch_from_torch / launch_from_slurm /
-launch_from_openmpi).  Design differences (B200-first):
+launch_from_openmpi).  Design differences (H100-first):
   * one process per GPU, NCCL on CUDA boxes, gloo on CPU boxes (the plumbing tier of the test-suite);
   * we do NOT force CUDA_DEVICE_MAX_CONNECTIONS=1 — overlap is obtained with explicit streams and fused
     compute+collective kernels rather than launch-order tricks;

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernel set (colossalai_b200).
+// Shared device helpers for the sm_90a kernel set (colossalai_b200).
 // Replaces the reference's csrc/funcs/*_functor.h + common/{micros,vec_type_traits,mp_type_traits}.h with a
 // much smaller surface: 16-byte vector I/O, fp32 math, warp/block reductions, and a runtime dtype switch.
 #pragma once
@@ -40,6 +40,16 @@ template <typename T> CB_DEVICE T from_f32(float v);
 template <> CB_DEVICE float from_f32<float>(float v) { return v; }
 template <> CB_DEVICE __half from_f32<__half>(float v) { return __float2half_rn(v); }
 template <> CB_DEVICE __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+// two consecutive elements <-> two floats (8-byte fp32 / 4-byte 16-bit accesses; the address is 2-element aligned)
+CB_DEVICE float2 to_f32x2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+CB_DEVICE float2 to_f32x2(const __nv_bfloat16* p) { return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p)); }
+CB_DEVICE float2 to_f32x2(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
+CB_DEVICE void store_f32x2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
+CB_DEVICE void store_f32x2(__nv_bfloat16* p, float a, float b) {
+  *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(a, b);
+}
+CB_DEVICE void store_f32x2(__half* p, float a, float b) { *reinterpret_cast<__half2*>(p) = __floats2half2_rn(a, b); }
 
 // A 16-byte vector of T (4 floats / 8 halves).
 template <typename T> struct Vec16 {
@@ -106,7 +116,7 @@ static inline int cb_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;   // H100 SXM
   }
   return n;
 }

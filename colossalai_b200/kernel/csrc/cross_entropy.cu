@@ -1,4 +1,4 @@
-// Fused (vocab-parallel) cross-entropy building blocks for sm_100a.
+// Fused (vocab-parallel) cross-entropy building blocks for sm_90a.
 // One CTA per token row; the [T, V_local] logits are streamed with 16-byte loads.  Forward reads the logits twice
 // (row max, then sum-exp relative to the GLOBAL max that python all-reduces in between); backward reads once and
 // writes the gradient once.  Replaces the eager torch composition in the reference's DistCrossEntropy

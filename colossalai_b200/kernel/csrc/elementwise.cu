@@ -1,4 +1,4 @@
-// Fused elementwise kernels for sm_100a: SwiGLU / GeGLU fwd+bwd on a packed [rows, 2*I] gate|up buffer,
+// Fused elementwise kernels for sm_90a: SwiGLU / GeGLU fwd+bwd on a packed [rows, 2*I] gate|up buffer,
 // RoPE (half-rotation layout) applied in place to the q and k head ranges of a packed QKV buffer (fwd and bwd),
 // bias+GELU fwd/bwd, bias+dropout+residual add, scale+inf/nan check.
 //

@@ -1,18 +1,20 @@
-// Fused compute + collective kernels for tensor / sequence parallel linears over NVLink peer memory (sm_100a).
+// Fused compute + collective kernels for tensor / sequence parallel linears over NVLink peer memory (sm_90a).
 //
 //   cb_ag_gemm   : Y[T, N]   = all_gather(x_local)[T, K] * B        (col-linear fwd under SP, and dX = AG(dY) * W)
 //   cb_gemm_rs   : y_local   = reduce_scatter(A[T, K] * B)          (row-linear fwd under SP, and dX of col-linear)
 //   cb_all_gather: X_full    = all_gather(x_local)                   (stand-alone pull, used for wgrad re-gather)
 //
-// One persistent launch does both jobs; the transfer overlaps the math tile by tile:
-//   * AG+GEMM: a few "copy CTAs" pull the peers' row chunks over NVLink (16-byte P2P loads from the peers' symmetric
-//     buffers) into the local gathered buffer, publishing one ready-flag per 128-row block; the remaining CTAs run the
-//     tcgen05/TMEM GEMM main loop and their TMA producer only waits for the flag of the A row-block it is about to load.
-//     Tiles are ordered local chunk first, then chunks in arrival order, so compute never idles while data is in flight.
-//   * GEMM+RS: every CTA runs the tcgen05 GEMM, writing bf16 partial tiles into a local symmetric buffer, chunk by
-//     chunk starting with the chunk owned by rank+1; when a rank finishes a chunk it signals the owner; the owner reduces
-//     its chunk straight out of the NVSwitch with multimem.ld_reduce (in-switch fp32 accumulation, falls back to P2P loads
-//     + adds when no multicast mapping exists) while other ranks are still computing later chunks.
+// One persistent launch does both jobs:
+//   * AG+GEMM (transfer overlapped with the math tile by tile): a few "copy warps" per CTA pull the peers' row chunks
+//     over NVLink (16-byte P2P loads from the peers' symmetric buffers) into the local gathered buffer, publishing one
+//     ready-flag per 128-row block; the wgmma GEMM main loop (gemm_sm90.cuh) runs in the same CTAs and its TMA producer
+//     only waits for the flag of the A row-block it is about to load.  Tiles are ordered local chunk first, then chunks
+//     in arrival order, so compute never idles while data is in flight.
+//   * GEMM+RS (transfer NOT overlapped with the math): every CTA runs the wgmma GEMM, writing bf16 partial tiles into a
+//     local symmetric buffer, chunk by chunk starting with the chunk owned by rank+1 (own chunk last); the last
+//     warpgroup to finish a chunk signals its owner.  After the GEMM, each rank waits until every peer has finished its
+//     chunk and reduces it straight out of the NVSwitch with multimem.ld_reduce (in-switch fp32 accumulation; P2P loads
+//     + adds when no multicast mapping exists).
 //   * cross-GPU ordering uses release/acquire at .sys scope on 32-bit epoch flags that live in symmetric memory; data
 //     written through the generic proxy and later read by TMA is fenced with fence.proxy.async on both sides.
 //
@@ -22,17 +24,16 @@
 #include <stdio.h>
 #include <stdlib.h>
 
-#include "common.cuh"
-#include "sm100.cuh"
+#include "gemm_sm90.cuh"
 
-using namespace sm100;
+using namespace sm90;
 
 namespace {
 
-constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int NUM_THREADS = 256;      // warps 0..5 = GEMM roles, warps 6..7 = NVLink pull (AG) / extra reduce lanes (RS)
+constexpr int BLOCK_M = gemm90::BM;
+constexpr int FIRST_COPY_WARP = gemm90::NUM_THREADS / 32;
+// warps 0..8 = GEMM roles (gemm_sm90.cuh), warps 9..10 = NVLink pull (AG) / extra reduce lanes (RS)
+constexpr int NUM_THREADS = gemm90::NUM_THREADS + 64;
 constexpr int COPY_WARPS = 2;
 constexpr int COPY_SEG = 8;           // a 128-row block is pulled as 8 segments of 16 rows by different warps
 constexpr int GROUP_M = 8;
@@ -43,17 +44,6 @@ constexpr int SLOT_IN_READY = 0;                 // [MAX_RANKS]  peer p wrote: "
 constexpr int SLOT_PULL_DONE = MAX_RANKS;        // [MAX_RANKS]  peer p wrote: "I finished reading your buffer (epoch e)"
 constexpr int SLOT_CHUNK_DONE = 2 * MAX_RANKS;   // [MAX_RANKS]  peer p wrote: "my partial of YOUR chunk is complete"
 constexpr int SLOT_LOCAL = 3 * MAX_RANKS;        // local scratch counters (never written by peers): [0..3]
-constexpr int SLOT_AR_DONE = 3 * MAX_RANKS + 4;  // [MAX_RANKS]  peer p wrote: "my chunk of the all-reduced output has
-                                                 // been broadcast into your copy (epoch e)"; page = 5 * MAX_RANKS words
-
-template <int BLOCK_N> struct Cfg {
-  static constexpr int STAGES = BLOCK_N == 256 ? 4 : 6;
-  static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 2 * BLOCK_N >= 512 ? 512 : 256;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-};
 
 struct CommParams {
   int rank, world;
@@ -73,50 +63,41 @@ struct CommParams {
   int ld_out;
   uint32_t* chunk_counter;           // RS: local per-chunk arrival counters [world]
   int out_dtype;
-  // RS, CTA-pair kernel: tile-granular pipeline (reduce of a tile starts as soon as every rank finished that tile)
-  uint32_t* peer_tile_flags[MAX_RANKS];  // symmetric [MAX_RANKS][tile_flag_stride] epoch flags (index = writer rank)
-  int tile_flag_stride;                  // flags per writer rank
-  uint32_t* tile_counter;                // local per-tile epilogue-warp arrival counters [m_blocks * n_blocks]
-  uint32_t* reduce_ticket;               // local work-queue head of the tile-granular reduction
-  uint32_t* rs_progress;                 // local per-slice progress words ((epoch << 5) | steps accumulated)
-  int rs_stream;                         // 1: uniform interleaved tile order + streamed in-switch reduction (below)
-  void* ar_out_mc;                       // GEMM+all-reduce: multicast address of the symmetric [T, N] output (or null)
 };
 
 struct GemmParams {
   int M, N, K;
   int ldc;
   int a_mn_major, b_mn_major;
-  uint32_t idesc;
   void* C;          // RS: local partial buffer (bf16); AG: output
   int out_dtype;
 };
 
 // ------------------------------------------------------------------------------------------- flag helpers
-SM100_DEVICE void st_release_sys(uint32_t* p, uint32_t v) {
+SM90_DEVICE void st_release_sys(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
-SM100_DEVICE uint32_t ld_acquire_sys(const uint32_t* p) {
+SM90_DEVICE uint32_t ld_acquire_sys(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-SM100_DEVICE void st_release_gpu(uint32_t* p, uint32_t v) {
+SM90_DEVICE void st_release_gpu(uint32_t* p, uint32_t v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
-SM100_DEVICE uint32_t ld_acquire_gpu(const uint32_t* p) {
+SM90_DEVICE uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-SM100_DEVICE void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-SM100_DEVICE bool epoch_reached(uint32_t v, uint32_t epoch) { return (int32_t)(v - epoch) >= 0; }
+SM90_DEVICE void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+SM90_DEVICE bool epoch_reached(uint32_t v, uint32_t epoch) { return (int32_t)(v - epoch) >= 0; }
 
 // Bounded spin on an epoch flag: a peer that never arrives (crashed rank, mismatched call sequence) must not hang the
 // GPU forever - after ~20 s the kernel reports and traps, which surfaces as a CUDA error in the host process.
 constexpr long long SPIN_TIMEOUT_CYCLES = 40LL * 1000 * 1000 * 1000;
 template <bool SYS>
-SM100_DEVICE void wait_epoch(const uint32_t* flag, uint32_t epoch) {
+SM90_DEVICE void wait_epoch(const uint32_t* flag, uint32_t epoch) {
   if (epoch_reached(SYS ? ld_acquire_sys(flag) : ld_acquire_gpu(flag), epoch)) return;
   const long long t0 = clock64();
   uint32_t it = 0;
@@ -130,27 +111,21 @@ SM100_DEVICE void wait_epoch(const uint32_t* flag, uint32_t epoch) {
   }
 }
 
-SM100_DEVICE uint4 ld_peer_16B(const void* p) {
+SM90_DEVICE uint4 ld_peer_16B(const void* p) {
   uint4 r;
   asm volatile("ld.global.relaxed.sys.v4.u32 {%0,%1,%2,%3}, [%4];"
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
   return r;
 }
 // in-switch reduction of 8 bf16 values held at the same offset on every rank (fp32 accumulate inside the NVSwitch)
-SM100_DEVICE uint4 multimem_ld_reduce_bf16x8(const void* mc_addr) {
+SM90_DEVICE uint4 multimem_ld_reduce_bf16x8(const void* mc_addr) {
   uint4 r;
   asm volatile("multimem.ld_reduce.relaxed.sys.global.add.acc::f32.v4.bf16x2 {%0,%1,%2,%3}, [%4];"
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(mc_addr) : "memory");
   return r;
 }
 
-// 16-byte store through the multicast mapping: the NVSwitch replicates it into every rank's copy of the buffer
-SM100_DEVICE void multimem_st_16B(void* mc_addr, const uint4& v) {
-  asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1,%2,%3,%4};"
-               :: "l"(mc_addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-SM100_DEVICE void tile_coords_rot(int tile, int m_blocks, int n_blocks, int m_rot, int& m_blk, int& n_blk) {
+SM90_DEVICE void tile_coords_rot(int tile, int m_blocks, int n_blocks, int m_rot, int& m_blk, int& n_blk) {
   const int tiles_per_group = GROUP_M * n_blocks;
   const int group = tile / tiles_per_group;
   const int first_m = group * GROUP_M;
@@ -161,31 +136,12 @@ SM100_DEVICE void tile_coords_rot(int tile, int m_blocks, int n_blocks, int m_ro
   m_blk = (m + m_rot) % m_blocks;     // rotate so the preferred chunk's row blocks come first
 }
 
-template <typename T16>
-SM100_DEVICE void store_chunk16(T16* __restrict__ dst, const uint32_t (&acc)[32], int n_valid) {
-  if (n_valid >= 32) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 8) {
-      Vec16<T16> o;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) o.set(i, __uint_as_float(acc[j + i]));
-      o.store(dst + j);
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j < n_valid) dst[j] = from_f32<T16>(__uint_as_float(acc[j]));
-  }
-}
-
-// NVLink pull executed by warps 6..7 of EVERY CTA (AG+GEMM): 16-row segments of the peers' chunks are copied into the
-// local gathered buffer, one ready flag per 128-row block is published once its 8 segments landed.
-SM100_DEVICE void ag_pull_warps(const CommParams& c, uint32_t* my_flags, int warp, int lane, int blocks_per_chunk) {
+SM90_DEVICE void ag_pull_warps(const CommParams& c, uint32_t* my_flags, int warp, int lane, int blocks_per_chunk) {
   // ================================================================ AG: NVLink pull by the copy warps of ALL CTAs
-  if (blockIdx.x == 0 && warp == 6 && lane < c.world)   // announce: my input buffer is valid for this epoch
+  if (blockIdx.x == 0 && warp == FIRST_COPY_WARP && lane < c.world)   // announce: my input buffer is valid for this epoch
     st_release_sys(c.peer_flags[lane] + SLOT_IN_READY + c.rank, c.epoch);
   const int vec_per_row = c.ld_in / 8;                  // 16-byte vectors per row
-  const int copy_warp = (int)blockIdx.x * COPY_WARPS + (warp - 6);
+  const int copy_warp = (int)blockIdx.x * COPY_WARPS + (warp - FIRST_COPY_WARP);
   const int n_copy_warps = (int)gridDim.x * COPY_WARPS;
   const int units_per_chunk = blocks_per_chunk * COPY_SEG;
   const int seg_rows = BLOCK_M / COPY_SEG;
@@ -249,7 +205,7 @@ SM100_DEVICE void ag_pull_warps(const CommParams& c, uint32_t* my_flags, int war
 
 // Reduce-scatter tail (GEMM+RS): after every peer signalled its partial of MY chunk, sum the chunk out of all partial
 // buffers (in-switch multimem reduction when a multicast mapping exists) and release the partial buffers.
-SM100_DEVICE void rs_reduce_phase(const GemmParams& p, const CommParams& c, uint32_t* my_flags) {
+SM90_DEVICE void rs_reduce_phase(const GemmParams& p, const CommParams& c, uint32_t* my_flags) {
   // ================================================================== RS: reduce MY chunk out of all partial buffers
   if (threadIdx.x < c.world) {
     wait_epoch<true>(my_flags + SLOT_CHUNK_DONE + threadIdx.x, c.epoch);
@@ -303,643 +259,86 @@ SM100_DEVICE void rs_reduce_phase(const GemmParams& p, const CommParams& c, uint
   }
 }
 
-// GEMM+RS, CTA-pair kernel: warps 6..7 of every CTA reduce MY chunk tile by tile while the GEMM roles are still
-// producing later tiles.  A 256 x 256 tile of my chunk is reduced (multimem.ld_reduce in the switch, or P2P loads) as soon
-// as every rank's partial of that tile is complete; the tiles of my chunk are visited in the order my own GEMM produces
-// them (they come last in the rotated tile order), so only the final tiles' reduction is exposed.
-// GEMM+RS, CTA-pair kernel: staggered pull-accumulate.
-// Rank q computes the chunks in the order q+1, q+2, ..., q, so the partial of MY chunk r becomes available on rank r-k
-// during time slot k (k = 1..world-1) and my own partial in the last slot.  Work units (32-row slices of the 256 x 256
-// tiles of my chunk, one per source rank) are handed out through a ticket counter in exactly that order: step k pulls
-// from rank r-k - a different NVLink peer per step, a permutation over the ranks, so every link is busy - and adds into
-// `out` (bf16 with fp32 adds: the precision of a ring reduce-scatter).  Warps 6..7 of every CTA take tickets from the
-// start (overlap with the main loop); warps 0..5 join when their GEMM role is finished, so a communication-bound
-// projection ends with all eight warps per SM pulling.  Step k of a slice waits for step k-1 of the same slice through
-// a per-slice progress word (tickets of step k-1 were issued earlier, so the wait is bounded).
-SM100_DEVICE void rs_reduce_tiles(const GemmParams& p, const CommParams& c, uint32_t* my_flags, int lane,
-                                  int m_blocks, int n_blocks, int pair_blocks_per_chunk, int m_rot, int total_warps) {
-  constexpr int SUB = 8;                                        // 32-row slices per 256-row tile
-  const int num_tiles = m_blocks * n_blocks;
-  const int tiles_per_chunk = pair_blocks_per_chunk * n_blocks;
-  const int n_units = tiles_per_chunk * SUB;
-  const uint32_t* my_tile_flags = c.peer_tile_flags[c.rank];
-  const size_t ldc_vec = p.ldc / 8;
-  const size_t ldo_vec = c.ld_out / 8;
-  const int my_first_blk = c.rank * pair_blocks_per_chunk;
-  const bool aligned = (pair_blocks_per_chunk % GROUP_M == 0);  // whole rasterisation groups per chunk
-  const uint32_t prog_base = c.epoch << 5;                      // progress word = (epoch << 5) | steps done
-  int scan_k = 0, scan_t = 0, scan_mine = 0, scan_m = 0, scan_n = 0;
-  while (true) {
-    int t = 0;
-    if (lane == 0) t = (int)atomicAdd(c.reduce_ticket, 1u);
-    t = __shfl_sync(0xffffffffu, t, 0);
-    if (t >= n_units * c.world) break;
-    const int k = t / n_units + 1;                              // 1 .. world (world = my own partial)
-    const int u = t - (k - 1) * n_units;
-    const int tile_in_chunk = u / SUB, sub = u - tile_in_chunk * SUB;
-    int m_blk, n_blk;
-    if (aligned) {
-      tile_coords_rot(num_tiles - tiles_per_chunk + tile_in_chunk, m_blocks, n_blocks, m_rot, m_blk, n_blk);
-    } else {
-      if (scan_k != k) { scan_k = k; scan_t = 0; scan_mine = 0; }
-      while (scan_mine <= tile_in_chunk && scan_t < num_tiles) {
-        int mb, nb;
-        tile_coords_rot(scan_t++, m_blocks, n_blocks, m_rot, mb, nb);
-        if (mb < my_first_blk || mb >= my_first_blk + pair_blocks_per_chunk) continue;
-        scan_m = mb; scan_n = nb;
-        ++scan_mine;
-      }
-      m_blk = scan_m; n_blk = scan_n;
-    }
-    const int src = (c.rank - k + 2 * c.world) % c.world;
-    const uint4* src_part = reinterpret_cast<const uint4*>(c.peer_part[src]);
-    const int slot = (m_blk - my_first_blk) * n_blocks + n_blk;
-    if (lane == 0) {
-      wait_epoch<true>(my_tile_flags + (size_t)src * c.tile_flag_stride + slot, c.epoch);     // partial tile exists
-      if (k > 1) wait_epoch<false>(c.rs_progress + u, prog_base + (uint32_t)(k - 1));          // previous step landed
-    }
-    __syncwarp();
-    const int col0 = n_blk * 256;
-    const int cols = min(256, p.N - col0);
-    const int vec_per_row = cols / 8;
-    const int row0 = m_blk * 256 + sub * 32;
-    const int rows = max(0, min(32, p.M - row0));
-    const int out_row0 = row0 - c.rank * c.rows_per_chunk;
-    const int nvec = rows * vec_per_row;
-    constexpr int RU = 16;                                      // 16 x 16 B peer loads in flight per lane
-    for (int i0 = lane; i0 < nvec; i0 += RU * 32) {
-      uint4 in[RU], cur[RU];
-      size_t doff[RU];
-#pragma unroll
-      for (int j = 0; j < RU; ++j) {
-        const int i = i0 + j * 32;
-        doff[j] = (size_t)-1;
-        if (i >= nvec) continue;
-        const int r = i / vec_per_row, cv = i - r * vec_per_row;
-        doff[j] = (size_t)(out_row0 + r) * ldo_vec + (col0 / 8) + cv;
-        in[j] = ld_peer_16B(src_part + (size_t)(row0 + r) * ldc_vec + (col0 / 8) + cv);
-      }
-      if (k > 1) {
-#pragma unroll
-        for (int j = 0; j < RU; ++j)
-          if (doff[j] != (size_t)-1) cur[j] = reinterpret_cast<const uint4*>(c.out)[doff[j]];
-      }
-#pragma unroll
-      for (int j = 0; j < RU; ++j) {
-        if (doff[j] == (size_t)-1) continue;
-        if (k > 1) {
-          Vec16<__nv_bfloat16> a, b2, o;
-          a.raw = in[j];
-          b2.raw = cur[j];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) o.set(e, a.get(e) + b2.get(e));
-          in[j] = o.raw;
-        }
-        reinterpret_cast<uint4*>(c.out)[doff[j]] = in[j];
-      }
-    }
-    __threadfence();
-    __syncwarp();
-    if (lane == 0) st_release_gpu(c.rs_progress + u, prog_base + (uint32_t)k);
-  }
-  // every partial buffer of this epoch has been consumed by me: the last warp of the grid resets the ticket and tells
-  // the peers that their partial buffers may be overwritten
-  __syncwarp();
-  if (lane == 0) {
-    const uint32_t done = atomicAdd(my_flags + SLOT_LOCAL + 1, 1u) + 1;
-    if (done == (uint32_t)total_warps) {
-      my_flags[SLOT_LOCAL + 1] = 0;
-      *c.reduce_ticket = 0;
-      __threadfence_system();
-      for (int r = 0; r < c.world; ++r) st_release_sys(c.peer_flags[r] + SLOT_PULL_DONE + c.rank, c.epoch);
-    }
-  }
-}
-
-// GEMM+RS, CTA-pair kernel, "stream" variant (CB200_RS_STREAM=1, needs the multicast mapping).
-// EVERY rank walks the output tiles in the same interleaved order - tile t belongs to chunk t % world and is the
-// (t / world)-th tile of that chunk - so the partials of tile j of chunk c complete on all ranks at about the same
-// time, and the owner of chunk c can reduce that tile INSIDE THE SWITCH (`multimem.ld_reduce`, fp32 accumulate) while
-// all ranks are already computing tile j+1.  The reduction streams through the whole GEMM instead of leaving the
-// owner's own partial for last (the problem of a rotated order), each output byte crosses NVLink once as a reduced
-// value, and only the last round of tiles is exposed.
-SM100_DEVICE void tile_coords_stream(int tile, int n_blocks, int pair_blocks_per_chunk, int world, int& m_blk,
-                                     int& n_blk) {
-  const int chunk = tile % world;
-  const int j = tile / world;
-  n_blk = j / pair_blocks_per_chunk;                 // consecutive tiles of a chunk share the B columns (L2 reuse)
-  m_blk = chunk * pair_blocks_per_chunk + (j - n_blk * pair_blocks_per_chunk);
-}
-
-SM100_DEVICE void rs_reduce_tiles_stream(const GemmParams& p, const CommParams& c, uint32_t* my_flags, int lane,
-                                         int n_blocks, int pair_blocks_per_chunk, int total_warps) {
-  constexpr int SUB = 8;                                        // 32-row slices per 256-row tile
-  const int tiles_per_chunk = pair_blocks_per_chunk * n_blocks;
-  const int n_units = tiles_per_chunk * SUB;
-  const uint32_t* my_tile_flags = c.peer_tile_flags[c.rank];
-  const size_t ldc_vec = p.ldc / 8;
-  const size_t ldo_vec = c.ld_out / 8;
-  const uint4* mc = reinterpret_cast<const uint4*>(c.mc_part);
-  // GEMM + ALL-REDUCE: the reduced tile is not kept for this rank only but stored through the multicast mapping of the
-  // symmetric [T, N] output, i.e. the switch broadcasts every reduced value to all ranks (reduce and broadcast both
-  // happen inside the NVSwitch; each output byte leaves this GPU once).
-  uint4* ar_mc = reinterpret_cast<uint4*>(c.ar_out_mc);
-  while (true) {
-    int t = 0;
-    if (lane == 0) t = (int)atomicAdd(c.reduce_ticket, 1u);
-    t = __shfl_sync(0xffffffffu, t, 0);
-    if (t >= n_units) break;
-    const int j = t / SUB, sub = t - j * SUB;
-    const int n_blk = j / pair_blocks_per_chunk;
-    const int mb = j - n_blk * pair_blocks_per_chunk;             // row block inside my chunk
-    const int slot = mb * n_blocks + n_blk;
-    if (lane < c.world)                                           // one lane per writer rank polls its (local) flag
-      wait_epoch<true>(my_tile_flags + (size_t)lane * c.tile_flag_stride + slot, c.epoch);
-    __syncwarp();
-    const int col0 = n_blk * 256;
-    const int cols = min(256, p.N - col0);
-    const int vec_per_row = cols / 8;
-    const int out_row0 = mb * 256 + sub * 32;                     // row inside my chunk == row of `out`
-    const int row0 = c.rank * c.rows_per_chunk + out_row0;        // row inside the [T, N] partial buffers
-    const int rows = max(0, min(32, c.rows_per_chunk - out_row0));
-    const int nvec = rows * vec_per_row;
-    constexpr int RU = 8;                                         // 8 switch reductions in flight per lane
-    for (int i0 = lane; i0 < nvec; i0 += RU * 32) {
-      uint4 v[RU];
-      size_t doff[RU];
-#pragma unroll
-      for (int q = 0; q < RU; ++q) {
-        const int i = i0 + q * 32;
-        doff[q] = (size_t)-1;
-        if (i >= nvec) continue;
-        const int r = i / vec_per_row, cv = i - r * vec_per_row;
-        doff[q] = ar_mc ? ((size_t)(row0 + r) * ldo_vec + (col0 / 8) + cv)
-                        : ((size_t)(out_row0 + r) * ldo_vec + (col0 / 8) + cv);
-        v[q] = multimem_ld_reduce_bf16x8(mc + (size_t)(row0 + r) * ldc_vec + (col0 / 8) + cv);
-      }
-#pragma unroll
-      for (int q = 0; q < RU; ++q) {
-        if (doff[q] == (size_t)-1) continue;
-        if (ar_mc) multimem_st_16B(ar_mc + doff[q], v[q]);
-        else reinterpret_cast<uint4*>(c.out)[doff[q]] = v[q];
-      }
-    }
-  }
-  __syncwarp();
-  if (lane == 0) {
-    if (ar_mc) __threadfence_system();                            // my broadcast stores are performed everywhere
-    const uint32_t done = atomicAdd(my_flags + SLOT_LOCAL + 1, 1u) + 1;
-    if (done == (uint32_t)total_warps) {
-      my_flags[SLOT_LOCAL + 1] = 0;
-      *c.reduce_ticket = 0;
-      __threadfence_system();
-      for (int r = 0; r < c.world; ++r) {
-        st_release_sys(c.peer_flags[r] + SLOT_PULL_DONE + c.rank, c.epoch);
-        if (ar_mc) st_release_sys(c.peer_flags[r] + SLOT_AR_DONE + c.rank, c.epoch);
-      }
-    }
-  }
-  if (ar_mc) {
-    // the kernel may only retire once EVERY rank's chunk has landed in this rank's copy of the output
-    if (lane < c.world) wait_epoch<true>(my_flags + SLOT_AR_DONE + lane, c.epoch);
-    __syncwarp();
-  }
-}
-
 // MODE 0: all-gather + GEMM.  MODE 1: GEMM + reduce-scatter.
-template <int BLOCK_N, int MODE>
+// The GEMM roles are those of gemm_sm90.cuh (warps 0..7 consumers, warp 8 producer); the tile order is rotated so the
+// preferred chunk comes first.  AG: the producer waits for the ready flag of the A row-block it is about to load.
+// RS: after storing its half of a partial tile a consumer warpgroup counts it for the chunk; the last one of a chunk
+// tells the chunk's owner.
+template <int MODE> struct FusedProb {
+  GemmParams p;
+  CommParams c;
+  int m_blocks, n_blocks, m_rot, blocks_per_chunk;
+  SM90_DEVICE int num_tiles() const { return m_blocks * n_blocks; }
+  SM90_DEVICE gemm90::Tile tile(int idx) const {
+    int m_blk, n_blk;
+    tile_coords_rot(idx, m_blocks, n_blocks, m_rot, m_blk, n_blk);
+    gemm90::Tile t;
+    t.a_mn0 = m_blk * BLOCK_M; t.a_k0 = 0;
+    t.b_mn0 = n_blk * gemm90::BN; t.b_k0 = 0;
+    t.k_blocks = (p.K + 63) / 64;
+    t.row0 = m_blk * BLOCK_M; t.row_lim = p.M;
+    t.col0 = n_blk * gemm90::BN; t.col_lim = p.N;
+    t.c_base = 0;
+    return t;
+  }
+  SM90_DEVICE void before_load(int, const gemm90::Tile& t) const {
+    if (MODE == 0) {
+      wait_epoch<false>(c.ready + t.a_mn0 / BLOCK_M, c.epoch);    // the A rows of this tile landed in `gathered`
+      fence_proxy_async_global();
+    }
+  }
+  SM90_DEVICE void after_store(int, const gemm90::Tile& t, int wg) const {
+    if (MODE != 1) return;
+    // publish: this warpgroup's half of the partial tile is globally visible; count tiles per chunk
+    __threadfence_system();
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if ((threadIdx.x & 127) == 0) {
+      const int chunk = (t.a_mn0 / BLOCK_M) / blocks_per_chunk;
+      const uint32_t got = atomicAdd(c.chunk_counter + chunk, 1u) + 1;
+      const uint32_t need = (uint32_t)blocks_per_chunk * n_blocks * 2;   // 2 consumer warpgroups per tile
+      if (got == need) {
+        c.chunk_counter[chunk] = 0;
+        __threadfence_system();
+        st_release_sys(c.peer_flags[chunk] + SLOT_CHUNK_DONE + c.rank, c.epoch);
+      }
+    }
+  }
+};
+
+template <int MODE, int A_MN, int B_MN, int KIND>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 fused_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const GemmParams p, const CommParams c) {
-  using C = Cfg<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + C::STAGES * C::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + C::STAGES;
-  uint64_t* tmem_full = bars + 2 * C::STAGES;
-  uint64_t* tmem_empty = bars + 2 * C::STAGES + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 4);
-
+  const gemm90::Smem s = gemm90::carve(smem_raw);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M;
-  const int n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = m_blocks * n_blocks;
-  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-  const int blocks_per_chunk = c.rows_per_chunk / BLOCK_M;
-  uint32_t* my_flags = c.peer_flags[c.rank];
-
-  const int gemm_cta = (int)blockIdx.x;
-  const int gemm_ctas = (int)gridDim.x;
-
-  // ==================================================================== GEMM roles
-  if (warp == 0 && lane == 0) {
-    prefetch_tensormap(&tmap_a);
-    prefetch_tensormap(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc<C::TMEM_COLS>(tmem_ptr_smem);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  FusedProb<MODE> prob;
+  prob.p = p;
+  prob.c = c;
+  prob.m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M;
+  prob.n_blocks = (p.N + gemm90::BN - 1) / gemm90::BN;
+  prob.blocks_per_chunk = c.rows_per_chunk / BLOCK_M;
   // AG: local chunk first.  RS: start with the chunk owned by rank+1, own chunk last.
-  const int m_rot = MODE == 0 ? c.rank * blocks_per_chunk : ((c.rank + 1) % c.world) * blocks_per_chunk;
-
-  if (warp == 0) {
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = gemm_cta; tile < num_tiles; tile += gemm_ctas) {
-      int m_blk, n_blk;
-      tile_coords_rot(tile, m_blocks, n_blocks, m_rot, m_blk, n_blk);
-      const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
-      if (MODE == 0) {
-        // the A rows of this tile must have landed in `gathered`
-        if (lane == 0) {
-          wait_epoch<false>(c.ready + m_blk, c.epoch);
-          fence_proxy_async_global();
-        }
-        __syncwarp();
-      }
-      for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (lane == 0) {
-          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-          uint8_t* sa = smem_a + stage * C::A_BYTES;
-          uint8_t* sb = smem_b + stage * C::B_BYTES;
-          const int k0 = kb * BLOCK_K;
-          if (!p.a_mn_major) {
-            tma_load_2d(&tmap_a, &full_bar[stage], sa, k0, m0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BLOCK_M / 64; ++j)
-              tma_load_2d(&tmap_a, &full_bar[stage], sa + j * (BLOCK_K * 128), m0 + j * 64, k0);
-          }
-          if (!p.b_mn_major) {
-            tma_load_2d(&tmap_b, &full_bar[stage], sb, k0, n0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BLOCK_N / 64; ++j)
-              tma_load_2d(&tmap_b, &full_bar[stage], sb + j * (BLOCK_K * 128), n0 + j * 64, k0);
-          }
-        }
-        __syncwarp();
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const uint32_t a_kstep = p.a_mn_major ? UMMA_K * 128 : UMMA_K * 2;
-    const uint32_t b_kstep = p.b_mn_major ? UMMA_K * 128 : UMMA_K * 2;
-    for (int tile = gemm_cta; tile < num_tiles; tile += gemm_ctas) {
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BLOCK_N;
-      for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = smem_u32(smem_a + stage * C::A_BYTES);
-          const uint32_t sb = smem_u32(smem_b + stage * C::B_BYTES);
-          const uint64_t da = p.a_mn_major ? make_smem_desc_sw128(sa, BLOCK_K * 128, 1024)
-                                           : make_smem_desc_sw128(sa, 16, 1024);
-          const uint64_t db = p.b_mn_major ? make_smem_desc_sw128(sb, BLOCK_K * 128, 1024)
-                                           : make_smem_desc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_f16_ss(tmem_d, advance_desc(da, k * a_kstep), advance_desc(db, k * b_kstep), p.idesc,
-                        (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (kb == k_blocks - 1) umma_commit(&tmem_full[acc]);
-        }
-        __syncwarp();
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else if (warp >= 6) {
-    if (MODE == 0) {
-      ag_pull_warps(c, my_flags, warp, lane, blocks_per_chunk);
-    }
-  } else {
-    const int quarter = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = gemm_cta; tile < num_tiles; tile += gemm_ctas) {
-      int m_blk, n_blk;
-      tile_coords_rot(tile, m_blocks, n_blocks, m_rot, m_blk, n_blk);
-      const int row = m_blk * BLOCK_M + quarter * 32 + lane;
-      const int n0 = n_blk * BLOCK_N;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * BLOCK_N + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-      for (int cc = 0; cc < BLOCK_N; cc += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + cc, v);
-        tmem_ld_wait();
-        const int n_valid = p.N - (n0 + cc);
-        if (row < p.M && n_valid > 0) {
-          const size_t off = (size_t)row * p.ldc + n0 + cc;
-          if (p.out_dtype == CB_BF16) store_chunk16<__nv_bfloat16>((__nv_bfloat16*)p.C + off, v, n_valid);
-          else store_chunk16<__half>((__half*)p.C + off, v, n_valid);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (MODE == 1) {
-        // publish: this warp's slice of the partial tile is globally visible; count tiles per chunk
-        __threadfence_system();
-        __syncwarp();
-        if (lane == 0) {
-          const int chunk = m_blk / blocks_per_chunk;
-          const uint32_t got = atomicAdd(c.chunk_counter + chunk, 1u) + 1;
-          const uint32_t need = (uint32_t)blocks_per_chunk * n_blocks * 4;   // 4 epilogue warps per tile
-          if (got == need) {
-            c.chunk_counter[chunk] = 0;
-            __threadfence_system();
-            st_release_sys(c.peer_flags[chunk] + SLOT_CHUNK_DONE + c.rank, c.epoch);
-          }
-        }
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<C::TMEM_COLS>(tmem_base);
-
-  if (MODE == 1) {
-    rs_reduce_phase(p, c, my_flags);
-  }
-}
-
-// =====================================================================================================================
-// CTA-pair (cta_group::2) version of the fused kernel: one 256 x 256 tile per cluster of two CTAs (see the plain kernel
-// in gemm_tcgen05.cu for the barrier topology).  Communication roles are unchanged: warps 6..7 of every CTA pull peer
-// rows (AG), every epilogue warp publishes its slice of a partial tile (RS).  Each CTA's TMA producer waits for the ready
-// flag of ITS OWN 128-row block of A, so the pair starts a tile as soon as both halves have landed.
-template <int BK_, int STAGES_> struct Cfg2 {
-  static constexpr int BK = BK_;
-  static constexpr int STAGES = STAGES_;
-  static constexpr int A_BYTES = 128 * BK * 2;
-  static constexpr int B_BYTES = 128 * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-};
-constexpr int PAIR_M = 256;
-constexpr int PAIR_N = 256;
-
-template <int MODE, int BK, int STAGES>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-fused_gemm_2cta_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                       const GemmParams p, const CommParams c) {
-  using C = Cfg2<BK, STAGES>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + C::STAGES * C::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + C::STAGES;
-  uint64_t* tmem_full = bars + 2 * C::STAGES;
-  uint64_t* tmem_empty = bars + 2 * C::STAGES + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
-  const int num_pairs = gridDim.x >> 1;
-  const int pair_id = blockIdx.x >> 1;
-  const int m_blocks = (p.M + PAIR_M - 1) / PAIR_M;            // 256-row blocks
-  const int n_blocks = (p.N + PAIR_N - 1) / PAIR_N;
-  const int num_tiles = m_blocks * n_blocks;
-  const int k_blocks = (p.K + BK - 1) / BK;
-  const int blocks_per_chunk = c.rows_per_chunk / BLOCK_M;     // 128-row blocks (flag granularity of the pull)
-  const int pair_blocks_per_chunk = c.rows_per_chunk / PAIR_M;
+  prob.m_rot = MODE == 0 ? c.rank * prob.blocks_per_chunk : ((c.rank + 1) % c.world) * prob.blocks_per_chunk;
   uint32_t* my_flags = c.peer_flags[c.rank];
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) gemm90::init_barriers(s);
+  if (warp == gemm90::PRODUCER_WARP && lane == 0) {
     prefetch_tensormap(&tmap_a);
     prefetch_tensormap(&tmap_b);
   }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8);
-    }
-    fence_barrier_init();
-  }
-  cluster_sync();
-  if (warp == 2) tmem_alloc_2cta<C::TMEM_COLS>(tmem_ptr_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const bool stream = MODE == 1 && c.rs_stream != 0;
-  const int m_rot = MODE == 0 ? c.rank * pair_blocks_per_chunk : ((c.rank + 1) % c.world) * pair_blocks_per_chunk;
-
-  if (warp == 0) {
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = pair_id; tile < num_tiles; tile += num_pairs) {
-      int m_blk, n_blk;
-      if (stream) tile_coords_stream(tile, n_blocks, pair_blocks_per_chunk, c.world, m_blk, n_blk);
-      else tile_coords_rot(tile, m_blocks, n_blocks, m_rot, m_blk, n_blk);
-      const int m0 = m_blk * PAIR_M + (int)cta_rank * 128;
-      const int n0 = n_blk * PAIR_N + (int)cta_rank * 128;
-      if (MODE == 0) {
-        if (lane == 0) {
-          wait_epoch<false>(c.ready + (m_blk * 2 + (int)cta_rank), c.epoch);
-          fence_proxy_async_global();
-        }
-        __syncwarp();
-      }
-      for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (lane == 0) {
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * C::STAGE_BYTES);
-          const uint32_t fb = map_to_cta(smem_u32(&full_bar[stage]), 0);
-          uint8_t* sa = smem_a + stage * C::A_BYTES;
-          uint8_t* sb = smem_b + stage * C::B_BYTES;
-          const int k0 = kb * BK;
-          if (!p.a_mn_major) {
-#pragma unroll
-            for (int j = 0; j < BK / 64; ++j) tma_load_2d_2sm(&tmap_a, fb, sa + j * (128 * 128), k0 + j * 64, m0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 2; ++j) tma_load_2d_2sm(&tmap_a, fb, sa + j * (BK * 128), m0 + j * 64, k0);
-          }
-          if (!p.b_mn_major) {
-#pragma unroll
-            for (int j = 0; j < BK / 64; ++j) tma_load_2d_2sm(&tmap_b, fb, sb + j * (128 * 128), k0 + j * 64, n0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 2; ++j) tma_load_2d_2sm(&tmap_b, fb, sb + j * (BK * 128), n0 + j * 64, k0);
-          }
-        }
-        __syncwarp();
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const uint32_t a_kstep = p.a_mn_major ? UMMA_K * 128 : UMMA_K * 2;
-      const uint32_t b_kstep = p.b_mn_major ? UMMA_K * 128 : UMMA_K * 2;
-      for (int tile = pair_id; tile < num_tiles; tile += num_pairs) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * PAIR_N;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (lane == 0) {
-            const uint32_t sa = smem_u32(smem_a + stage * C::A_BYTES);
-            const uint32_t sb = smem_u32(smem_b + stage * C::B_BYTES);
-            const uint64_t da = p.a_mn_major ? make_smem_desc_sw128(sa, BK * 128, 1024)
-                                             : make_smem_desc_sw128(sa, 16, 1024);
-            const uint64_t db = p.b_mn_major ? make_smem_desc_sw128(sb, BK * 128, 1024)
-                                             : make_smem_desc_sw128(sb, 16, 1024);
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint32_t ao = p.a_mn_major ? k * a_kstep : (k >> 2) * (128 * 128) + (k & 3) * a_kstep;
-              const uint32_t bo = p.b_mn_major ? k * b_kstep : (k >> 2) * (128 * 128) + (k & 3) * b_kstep;
-              umma_f16_ss_2cta(tmem_d, advance_desc(da, ao), advance_desc(db, bo), p.idesc,
-                               (kb > 0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit_2cta(&empty_bar[stage], 3);
-            if (kb == k_blocks - 1) umma_commit_2cta(&tmem_full[acc], 3);
-          }
-          __syncwarp();
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 6) {
-    if (MODE == 0) ag_pull_warps(c, my_flags, warp, lane, blocks_per_chunk);
+  const int num_tiles = prob.num_tiles();
+  if (warp >= FIRST_COPY_WARP) {
+    if (MODE == 0) ag_pull_warps(c, my_flags, warp, lane, prob.blocks_per_chunk);
+  } else if (warp == gemm90::PRODUCER_WARP) {
+    gemm90::producer<KIND, A_MN, B_MN>(&tmap_a, &tmap_b, prob, s, num_tiles);
   } else {
-    const int quarter = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = pair_id; tile < num_tiles; tile += num_pairs) {
-      int m_blk, n_blk;
-      if (stream) tile_coords_stream(tile, n_blocks, pair_blocks_per_chunk, c.world, m_blk, n_blk);
-      else tile_coords_rot(tile, m_blocks, n_blocks, m_rot, m_blk, n_blk);
-      const int row = m_blk * PAIR_M + (int)cta_rank * 128 + quarter * 32 + lane;
-      const int n0 = n_blk * PAIR_N;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * PAIR_N + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-      for (int cc = 0; cc < PAIR_N; cc += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + cc, v);
-        tmem_ld_wait();
-        const int n_valid = p.N - (n0 + cc);
-        if (row < p.M && n_valid > 0) {
-          const size_t off = (size_t)row * p.ldc + n0 + cc;
-          if (p.out_dtype == CB_BF16) store_chunk16<__nv_bfloat16>((__nv_bfloat16*)p.C + off, v, n_valid);
-          else store_chunk16<__half>((__half*)p.C + off, v, n_valid);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tmem_empty[acc]);
-        else mbar_arrive_cluster(map_to_cta(smem_u32(&tmem_empty[acc]), 0));
-      }
-      if (MODE == 1) {
-        __threadfence_system();
-        __syncwarp();
-        if (lane == 0) {
-          // tile-granular publication: the 8th epilogue warp (2 CTAs x 4) of a tile tells the chunk owner
-          const int chunk = m_blk / pair_blocks_per_chunk;
-          uint32_t* ctr = c.tile_counter + (size_t)m_blk * n_blocks + n_blk;
-          const uint32_t got = atomicAdd(ctr, 1u) + 1;
-          if (got == 8u) {
-            *ctr = 0;
-            __threadfence_system();
-            const int slot = (m_blk - chunk * pair_blocks_per_chunk) * n_blocks + n_blk;
-            st_release_sys(c.peer_tile_flags[chunk] + (size_t)c.rank * c.tile_flag_stride + slot, c.epoch);
-          }
-        }
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    const gemm90::Epilogue e{p.C, p.ldc, p.out_dtype, 0, nullptr, nullptr};
+    gemm90::consumer<KIND, A_MN, B_MN>(prob, s, e, num_tiles);
   }
-  if (MODE == 1) {   // warps 6..7 arrive here at once, the GEMM roles when their tiles are done
-    if (stream) rs_reduce_tiles_stream(p, c, my_flags, lane, n_blocks, pair_blocks_per_chunk, (int)gridDim.x * 8);
-    else rs_reduce_tiles(p, c, my_flags, lane, m_blocks, n_blocks, pair_blocks_per_chunk, m_rot, (int)gridDim.x * 8);
-  }
-  tc_fence_before();
-  cluster_sync();
-  if (warp == 2) tmem_dealloc_2cta<C::TMEM_COLS>(tmem_base);
-}
-
-template <int MODE, int BK = 128, int STAGES = 3>
-int launch_fused_2cta(const void* A, const void* B, int M, int N, int K, int lda, int ldb, int a_mn, int b_mn,
-                      int in_dtype, GemmParams p, const CommParams& c, cudaStream_t stream) {
-  using C = Cfg2<BK, STAGES>;
-  CUtensorMap ta, tb;
-  const bool bf16 = in_dtype == CB_BF16;
-  int r = a_mn ? make_tmap_2d_16b(&ta, A, K, M, lda, BK, 64, bf16) : make_tmap_2d_16b(&ta, A, M, K, lda, 128, 64, bf16);
-  if (r) return 1000 + r;
-  r = b_mn ? make_tmap_2d_16b(&tb, B, K, N, ldb, BK, 64, bf16) : make_tmap_2d_16b(&tb, B, N, K, ldb, 128, 64, bf16);
-  if (r) return 2000 + r;
-  p.idesc = make_idesc_f16(PAIR_M, PAIR_N, bf16 ? 1 : 0, a_mn, b_mn);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(fused_gemm_2cta_kernel<MODE, BK, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         C::SMEM_BYTES);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
-  const int grid = cb_num_sms() & ~1;     // all CTAs co-resident (flag spinning): one CTA per SM, whole pairs
-  fused_gemm_2cta_kernel<MODE, BK, STAGES><<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, p, c);
-  return (int)cudaGetLastError();
-}
-
-// CTA-pair kernels need whole 256-row blocks per rank chunk
-inline bool use_pair_kernel(int T, int world, int N, int block_n) {
-  static int enabled = -1;
-  if (enabled < 0) {
-    const char* e = getenv("CB200_FUSED_2CTA");
-    enabled = e ? atoi(e) : 1;
-  }
-  if (block_n == 512) return true;
-  return enabled && block_n == 0 && (T / world) % PAIR_M == 0 && N >= 256;
+  __syncthreads();
+  if (MODE == 1) rs_reduce_phase(p, c, my_flags);
 }
 
 // Stand-alone all-gather by P2P pull (every CTA is a copy CTA).
@@ -974,7 +373,7 @@ __global__ void __launch_bounds__(256) all_gather_pull_kernel(const CommParams c
 // Stand-alone reduce-scatter over symmetric memory: every rank has written its full [world * rows_per_chunk, ld] input
 // into its symmetric buffer; rank r sums chunk r over all ranks (fp32 accumulation: in-switch `multimem.ld_reduce` when a
 // multicast mapping exists, otherwise 16-byte P2P loads) and writes it to `out`.  ELEM: 0 = bf16, 1 = fp32.
-SM100_DEVICE uint4 multimem_ld_reduce_f32x4(const void* mc_addr) {
+SM90_DEVICE uint4 multimem_ld_reduce_f32x4(const void* mc_addr) {
   uint4 r;
   asm volatile("multimem.ld_reduce.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4];"
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(mc_addr) : "memory");
@@ -1106,28 +505,39 @@ __global__ void wait_pull_done_kernel(uint32_t* my_flags, int world, uint32_t ep
     wait_epoch<true>(my_flags + SLOT_PULL_DONE + threadIdx.x, epoch);
 }
 
-template <int BLOCK_N, int MODE>
-int launch_fused(const void* A, const void* B, int M, int N, int K, int lda, int ldb, int a_mn, int b_mn, int in_dtype,
-                 GemmParams p, const CommParams& c, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N>;
-  CUtensorMap ta, tb;
-  const bool bf16 = in_dtype == CB_BF16;
-  int r = a_mn ? make_tmap_2d_16b(&ta, A, K, M, lda, BLOCK_K, 64, bf16) : make_tmap_2d_16b(&ta, A, M, K, lda, BLOCK_M, 64, bf16);
-  if (r) return 1000 + r;
-  r = b_mn ? make_tmap_2d_16b(&tb, B, K, N, ldb, BLOCK_K, 64, bf16) : make_tmap_2d_16b(&tb, B, N, K, ldb, BLOCK_N, 64, bf16);
-  if (r) return 2000 + r;
-  p.idesc = make_idesc_f16(BLOCK_M, BLOCK_N, bf16 ? 1 : 0, a_mn, b_mn);
+template <int MODE, int A_MN, int B_MN, int KIND>
+int launch_fused_k(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, const CommParams& c,
+                   cudaStream_t stream) {
+  constexpr int SMEM = gemm90::SMEM_BYTES;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(fused_gemm_kernel<BLOCK_N, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         C::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(fused_gemm_kernel<MODE, A_MN, B_MN, KIND>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
   // persistent grid: ALL CTAs must be co-resident (flag spinning) -> exactly one CTA per SM
-  const int grid = cb_num_sms();
-  fused_gemm_kernel<BLOCK_N, MODE><<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, p, c);
+  fused_gemm_kernel<MODE, A_MN, B_MN, KIND><<<cb_num_sms(), NUM_THREADS, SMEM, stream>>>(ta, tb, p, c);
   return (int)cudaGetLastError();
+}
+
+template <int MODE>
+int launch_fused(const void* A, const void* B, int M, int N, int K, int lda, int ldb, int a_mn, int b_mn, int in_dtype,
+                 GemmParams p, const CommParams& c, cudaStream_t stream) {
+  CUtensorMap ta, tb;
+  const bool bf16 = in_dtype == CB_BF16;
+  int r = gemm90::tmap16(&ta, A, a_mn, M, K, lda, bf16);
+  if (r) return 1000 + r;
+  r = gemm90::tmap16(&tb, B, b_mn, N, K, ldb, bf16);
+  if (r) return 2000 + r;
+#define CB_F(A_, B_)                                                                     \
+  return bf16 ? launch_fused_k<MODE, A_, B_, gemm90::K_BF16>(ta, tb, p, c, stream)       \
+              : launch_fused_k<MODE, A_, B_, gemm90::K_F16>(ta, tb, p, c, stream)
+  if (!a_mn && !b_mn) CB_F(0, 0);
+  if (!a_mn && b_mn) CB_F(0, 1);
+  if (a_mn && !b_mn) CB_F(1, 0);
+  CB_F(1, 1);
+#undef CB_F
 }
 
 }  // namespace
@@ -1151,12 +561,8 @@ int cb_ag_gemm(const void* const* peer_in, uint32_t* const* peer_flags, void* ga
   c.gathered = gathered; c.ld_in = K; c.ready = ready; c.block_counter = block_counter;
   GemmParams p{};
   p.M = T; p.N = N; p.K = K; p.ldc = ldy; p.a_mn_major = 0; p.b_mn_major = b_mn_major; p.C = Y; p.out_dtype = in_dtype;
-  if (use_pair_kernel(T, world, N, block_n) && (T / world) % PAIR_M == 0)
-    return launch_fused_2cta<0>(gathered, B, T, N, K, K, ldb, 0, b_mn_major, in_dtype, p, c, stream);
-  if (block_n == 0 || block_n == 512) block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
-  if (block_n == 256)
-    return launch_fused<256, 0>(gathered, B, T, N, K, K, ldb, 0, b_mn_major, in_dtype, p, c, stream);
-  return launch_fused<128, 0>(gathered, B, T, N, K, K, ldb, 0, b_mn_major, in_dtype, p, c, stream);
+  (void)block_n;
+  return launch_fused<0>(gathered, B, T, N, K, K, ldb, 0, b_mn_major, in_dtype, p, c, stream);
 }
 
 // y_local[T/world, N] = reduce_scatter_rows( A[T, K] (x) B ).  `part` is this rank's symmetric [T, N] partial buffer,
@@ -1164,9 +570,7 @@ int cb_ag_gemm(const void* const* peer_in, uint32_t* const* peer_flags, void* ga
 int cb_gemm_rs(const void* A, const void* B, void* part, const void* const* peer_part, const void* mc_part,
                uint32_t* const* peer_flags, uint32_t* chunk_counter, void* out, int T, int N, int K, int lda, int ldb,
                int ld_out, int a_mn_major, int b_mn_major, int in_dtype, int rank, int world, uint32_t epoch,
-               int block_n, uint32_t* const* peer_tile_flags, int tile_flag_stride, uint32_t* tile_counter,
-               int tile_counter_len, uint32_t* rs_progress, int rs_progress_len, int rs_variant, void* ar_out_mc,
-               cudaStream_t stream) {
+               int block_n, cudaStream_t stream) {
   if (world > MAX_RANKS || T % (world * BLOCK_M) != 0 || N % 8 != 0) return (int)cudaErrorInvalidValue;
   CommParams c{};
   c.rank = rank; c.world = world; c.epoch = epoch; c.rows_per_chunk = T / world;
@@ -1175,35 +579,8 @@ int cb_gemm_rs(const void* A, const void* B, void* part, const void* const* peer
   GemmParams p{};
   p.M = T; p.N = N; p.K = K; p.ldc = N; p.a_mn_major = a_mn_major; p.b_mn_major = b_mn_major; p.C = part;
   p.out_dtype = in_dtype;
-  const int pair_tiles_chunk = ((T / world) / PAIR_M) * ((N + PAIR_N - 1) / PAIR_N);
-  const int pair_tiles = (T / PAIR_M) * ((N + PAIR_N - 1) / PAIR_N);
-  if (use_pair_kernel(T, world, N, block_n) && (T / world) % PAIR_M == 0 && peer_tile_flags && tile_counter &&
-      rs_progress && pair_tiles_chunk * 8 <= rs_progress_len && epoch < (1u << 26) &&
-      pair_tiles_chunk <= tile_flag_stride && pair_tiles < tile_counter_len) {
-    for (int r = 0; r < world; ++r) c.peer_tile_flags[r] = peer_tile_flags[r];
-    c.tile_flag_stride = tile_flag_stride;
-    c.tile_counter = tile_counter;
-    c.reduce_ticket = tile_counter + (tile_counter_len - 1);
-    c.rs_progress = rs_progress;
-    // CB200_RS_STREAM=1: uniform tile order + streamed in-switch reduction (bf16 partials, multicast mapping needed)
-    // rs_variant: 0 = env default (CB200_RS_STREAM), 1 = staggered P2P pull-accumulate, 2 = streamed in-switch reduce
-    static int rs_stream_env = -1;
-    if (rs_stream_env < 0) {
-      const char* e = getenv("CB200_RS_STREAM");
-      rs_stream_env = e ? atoi(e) : 0;
-    }
-    const bool want_stream = rs_variant == 2 || (rs_variant == 0 && rs_stream_env);
-    const bool can_stream = mc_part != nullptr && in_dtype == CB_BF16 && N % 256 == 0;
-    if ((rs_variant == 2 || ar_out_mc) && !can_stream) return (int)cudaErrorInvalidValue;
-    c.rs_stream = (want_stream || ar_out_mc) ? 1 : 0;
-    c.ar_out_mc = ar_out_mc;
-    return launch_fused_2cta<1>(A, B, T, N, K, lda, ldb, a_mn_major, b_mn_major, in_dtype, p, c, stream);
-  }
-  if (rs_variant == 2 || ar_out_mc) return (int)cudaErrorInvalidValue;   // only the CTA-pair kernel streams
-  if (block_n == 0 || block_n == 512) block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
-  if (block_n == 256)
-    return launch_fused<256, 1>(A, B, T, N, K, lda, ldb, a_mn_major, b_mn_major, in_dtype, p, c, stream);
-  return launch_fused<128, 1>(A, B, T, N, K, lda, ldb, a_mn_major, b_mn_major, in_dtype, p, c, stream);
+  (void)block_n;
+  return launch_fused<1>(A, B, T, N, K, lda, ldb, a_mn_major, b_mn_major, in_dtype, p, c, stream);
 }
 
 int cb_all_gather_pull(const void* const* peer_in, uint32_t* const* peer_flags, void* gathered, int rows_per_chunk,

@@ -1,4 +1,4 @@
-// Paged-KV inference kernels for sm_100a.
+// Paged-KV inference kernels for sm_90a.
 //
 // KV cache layout (both K and V, per layer):  [num_blocks, block_size, kv_heads, head_dim]  (token-major inside a block,
 // 16-byte vectors along head_dim; one (block, head) tile is a strided 2-D box, i.e. directly TMA-addressable).
@@ -17,7 +17,7 @@
 // decode_kv_cache_memcpy,context_kv_cache_memcpy,fused_rotary_emb_and_cache,get_cos_and_sin,convert_fp8}_kernel.cu,
 // N12-N19) and the Triton twins (kernel/triton/{flash_decoding,kvcache_copy,no_pad_rotary_embedding}.py).
 // Decode attention is HBM-bound (every K/V byte is read once): the design goal is full-sector 16-byte loads, many of them
-// in flight per SM, and enough CTAs (seqs x kv_heads x splits >= 2 waves of 2 x 148) rather than tensor cores.
+// in flight per SM, and enough CTAs (seqs x kv_heads x splits >= 2 waves of 2 x 132 on an H100) rather than tensor cores.
 #include "common.cuh"
 
 namespace {

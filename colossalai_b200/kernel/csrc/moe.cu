@@ -1,4 +1,4 @@
-// Mixture-of-experts kernels for sm_100a.
+// Mixture-of-experts kernels for sm_90a.
 //
 //  (1) capacity-based dispatch / combine (+ cumsum) used by the legacy top-1 / top-2 MoE layer.  Behavioural parity:
 //      reference extensions/csrc/kernel/cuda/moe_kernel.cu (moe_dispatch_fwd/bwd, moe_combine_fwd/bwd, cumsum_sub_one).
@@ -523,13 +523,13 @@ int cb_moe_ep_dispatch(const void* x, const int* topk_idx, const void* const* ro
   cudaMemsetAsync(cursor, 0, sizeof(int) * E, st);
   if (n > 0) {
     int g = (n + 1023) / 1024;
-    if (g > 148) g = 148;
+    if (g > cb_num_sms()) g = cb_num_sms();
     ep_histogram_kernel<<<g, 256, E * sizeof(int), st>>>(topk_idx, n, E, counts_local);
   }
   ep_exchange_counts_kernel<<<1, 256, 2 * E * sizeof(int), st>>>(p, counts_local, send_off, local_counts, local_offs,
                                                                  real_counts, meta);
   int grid = (n + 7) / 8;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > cb_num_sms() * 4) grid = cb_num_sms() * 4;
   if (grid < 1) grid = 1;
   CB_DISPATCH_HALF(dtype, T, {
     ep_push_rows_kernel<T><<<grid, 256, 0, st>>>(p, (const T*)x, topk_idx, nullptr, send_off, cursor, pos, n, K, H,
@@ -543,7 +543,7 @@ int cb_moe_ep_dispatch(const void* x, const int* topk_idx, const void* const* ro
 int cb_moe_ep_take_rows(void* dst, const void* src, int64_t row_bytes, const int* local_offs, const int* real_counts,
                         int n_local, int max_rows, cudaStream_t st) {
   if (row_bytes % 16 != 0 || n_local < 1) return (int)cudaErrorInvalidValue;
-  ep_take_rows_kernel<<<148 * 4, 256, 0, st>>>((uint4*)dst, (const uint4*)src, (int)(row_bytes / 16), local_offs,
+  ep_take_rows_kernel<<<cb_num_sms() * 4, 256, 0, st>>>((uint4*)dst, (const uint4*)src, (int)(row_bytes / 16), local_offs,
                                                real_counts, n_local, max_rows);
   return CB_LAUNCH_CHECK();
 }
@@ -556,7 +556,7 @@ int cb_moe_ep_push_known(const void* x, const int* topk_idx, const float* scale,
   EpParams p = make_ep(rows, flags, nullptr, rank, world, E, 0, epoch);
   const int n = tokens * K;
   int grid = (n + 7) / 8;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > cb_num_sms() * 4) grid = cb_num_sms() * 4;
   if (grid < 1) grid = 1;
   CB_DISPATCH_HALF(dtype, T, {
     ep_push_rows_kernel<T><<<grid, 256, 0, st>>>(p, (const T*)x, topk_idx, scale, nullptr, nullptr,
@@ -574,7 +574,7 @@ int cb_moe_ep_combine(const int* topk_idx, const float* w, const int* pos, const
   EpParams p = make_ep(rows, flags, nullptr, rank, world, E, 0, epoch);
   ep_signal_kernel<<<1, 32, 0, st>>>(p, SLOT_Y);
   int grid = (tokens + 7) / 8;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > cb_num_sms() * 4) grid = cb_num_sms() * 4;
   if (grid < 1) grid = 1;
   CB_DISPATCH_HALF(dtype, T, {
     ep_pull_combine_kernel<T><<<grid, 256, 0, st>>>(p, topk_idx, w, pos, (T*)out, (T*)ys_keep, tokens, K, H);

@@ -1,4 +1,4 @@
-// Multi-tensor optimizer kernels for sm_100a: Adam/AdamW (fp32 master + low-precision working copy written in the
+// Multi-tensor optimizer kernels for sm_90a: Adam/AdamW (fp32 master + low-precision working copy written in the
 // same pass, fused grad un-scale / clip), SGD(+momentum, nesterov), LAMB (two stages), L2/max norm, scale+inf check.
 //
 // Capability parity: reference fused_optim_cuda (extensions/csrc/kernel/cuda/multi_tensor_{adam,sgd,lamb,l2norm,

@@ -1,4 +1,4 @@
-// Fused RMSNorm / LayerNorm forward + backward for sm_100a (memory-bound: 16-byte vector I/O, row in registers,
+// Fused RMSNorm / LayerNorm forward + backward for sm_90a (memory-bound: 16-byte vector I/O, row in registers,
 // fp32 statistics, one pass over HBM per tensor).
 //
 // Capability parity: reference apex FusedRMSNorm/FusedLayerNorm usage (shardformer/layer/normalization.py:27-135),

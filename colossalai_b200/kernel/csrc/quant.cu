@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(512) cast_from_fp8_kernel(const uint8_t* __res
 
 inline int grid_for(int64_t n, int per_block) {
   int64_t g = (n + per_block - 1) / per_block;
-  return (int)(g < 1 ? 1 : (g > 148 * 8 ? 148 * 8 : g));
+  return (int)(g < 1 ? 1 : (g > cb_num_sms() * 8 ? cb_num_sms() * 8 : g));
 }
 
 }  // namespace

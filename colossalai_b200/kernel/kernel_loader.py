@@ -1,7 +1,7 @@
 """`KernelLoader` façade over the native library loader.
 
 Parity: reference `colossalai/kernel/kernel_loader.py:32-120` (`KernelLoader.load()` picks the first available
-extension for the device; one subclass per kernel family).  Here every family maps to one in-tree sm_100a library
+extension for the device; one subclass per kernel family).  Here every family maps to one in-tree sm_90a library
 (`kernel/loader.py`); `load()` returns the ctypes handle and raises if the library cannot be built/loaded.
 """
 from __future__ import annotations

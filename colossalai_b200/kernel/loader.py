@@ -1,8 +1,8 @@
 """Native kernel build + load.
 
 Parity: reference `colossalai/kernel/kernel_loader.py:31-131` + `extensions/{base,cpp,cuda}_extension.py`
-(AOT/JIT build of op families, `KernelLoader.load()`).  B200-first differences:
-  * ONE arch: every `.cu` is compiled with `-gencode arch=compute_100a,code=sm_100a -lineinfo`;
+(AOT/JIT build of op families, `KernelLoader.load()`).  H100-first differences:
+  * ONE arch: every `.cu` is compiled with `-gencode arch=compute_90a,code=sm_90a -lineinfo`;
   * kernels export plain C launchers (`extern "C"`, raw pointers + cudaStream_t) and are loaded with ctypes —
     no torch headers in the CUDA translation units, so a full rebuild takes seconds and the `.so` files live
     IN-TREE (`colossalai_b200/kernel/_build/`) so they travel to the GPU box with the repo snapshot;
@@ -29,7 +29,7 @@ CSRC = _HERE / "csrc"
 BUILD = _HERE / "_build"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math",
     "--expt-relaxed-constexpr", "--expt-extended-lambda", "-Xcompiler", "-fPIC", "-shared",
     "-U__CUDA_NO_HALF_OPERATORS__", "-U__CUDA_NO_HALF_CONVERSIONS__", "-U__CUDA_NO_BFLOAT16_CONVERSIONS__",
     "-U__CUDA_NO_HALF2_OPERATORS__",
@@ -43,9 +43,9 @@ LIBS: Dict[str, dict] = {
     "cb200_optim": {"sources": ["multi_tensor_optim.cu"], "kind": "cuda"},
     "cb200_softmax": {"sources": ["softmax.cu"], "kind": "cuda"},
     "cb200_loss": {"sources": ["cross_entropy.cu"], "kind": "cuda"},
-    "cb200_gemm": {"sources": ["gemm_tcgen05.cu"], "kind": "cuda"},
-    "cb200_grouped_gemm": {"sources": ["grouped_gemm_tcgen05.cu"], "kind": "cuda"},
-    "cb200_attn": {"sources": ["flash_attn_tcgen05.cu"], "kind": "cuda"},
+    "cb200_gemm": {"sources": ["gemm_wgmma.cu"], "kind": "cuda"},
+    "cb200_grouped_gemm": {"sources": ["grouped_gemm_wgmma.cu"], "kind": "cuda"},
+    "cb200_attn": {"sources": ["flash_attn_wgmma.cu"], "kind": "cuda"},
     "cb200_comm": {"sources": ["fused_comm_gemm.cu"], "kind": "cuda"},
     "cb200_moe": {"sources": ["moe.cu"], "kind": "cuda"},
     "cb200_infer": {"sources": ["inference.cu"], "kind": "cuda"},

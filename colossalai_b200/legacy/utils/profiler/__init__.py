@@ -31,7 +31,7 @@ class BaseProfiler:
 
 class PcieProfiler(BaseProfiler):
     """Host<->device copy profiler: records every `Memcpy HtoD / DtoH` of a `torch.profiler` trace with bytes, time
-    and achieved bandwidth (on B200 boxes this is the Gen5 x16 / C2C link the offload paths ride on)."""
+    and achieved bandwidth (the PCIe link the offload paths ride on)."""
 
     def __init__(self, dtype: str = "fp32", depth: int = 1) -> None:
         super().__init__("Pcie", 10)

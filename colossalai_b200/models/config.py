@@ -164,6 +164,11 @@ MODEL_ZOO: Dict[str, ModelConfig] = {
     "llama3-8b": _llama(vocab_size=128256, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
                         num_attention_heads=32, num_key_value_heads=8, max_position_embeddings=8192,
                         rope_theta=500000.0),
+    # Llama-3.2-1B shape (untied head): the largest Llama-3 that trains with fp32 master weights and AdamW moments on
+    # one 80 GB GPU without offload
+    "llama3.2-1b": _llama(vocab_size=128256, hidden_size=2048, intermediate_size=8192, num_hidden_layers=16,
+                          num_attention_heads=32, num_key_value_heads=8, max_position_embeddings=8192,
+                          rope_theta=500000.0),
     "llama3-70b": _llama(vocab_size=128256, hidden_size=8192, intermediate_size=28672, num_hidden_layers=80,
                          num_attention_heads=64, num_key_value_heads=8, max_position_embeddings=8192,
                          rope_theta=500000.0),

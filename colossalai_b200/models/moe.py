@@ -1,7 +1,7 @@
 """Sparse Mixture-of-Experts block with expert parallelism (Mixtral / DeepSeekMoE / DeepSeek-V3 routing).
 
 Parity: reference `EPMixtralSparseMoeBlock` (`colossalai/shardformer/modeling/mixtral.py:54-208`), `EPDeepseekMoE`
-(`deepseek.py:63-230`), `EpDeepseekV3MoE` (`deepseek_v3.py:26`).  Differences (B200-first):
+(`deepseek.py:63-230`), `EpDeepseekV3MoE` (`deepseek_v3.py:26`).  Differences (H100-first):
   * expert weights are batched tensors `[E_local, 2I, H]` / `[E_local, H, I]` driven by ONE grouped GEMM per
     projection instead of a python loop of small GEMMs;
   * dispatch/combine go through `colossalai_b200.moe` which has two backends: `nccl` (sorted tokens + uneven

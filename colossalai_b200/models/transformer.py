@@ -54,7 +54,7 @@ class SeqMeta:
 
 
 def _use_fused_a2a(x: torch.Tensor, sp_group) -> bool:
-    """Ulysses all-to-all through the sm_100a pull kernel: CUDA tensors under the `fused` comm backend."""
+    """Ulysses all-to-all through the sm_90a pull kernel: CUDA tensors under the `fused` comm backend."""
     from ..shardformer.layer._operation import get_comm_backend
 
     if not x.is_cuda or get_comm_backend() != "fused" or comm.group_size(sp_group) == 1:

@@ -50,7 +50,7 @@ def _aligned_rows(x: torch.Tensor) -> bool:
     weight-gradient GEMM then needs no re-layout pass (moe/grouped_gemm.py)."""
     return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16)
             and os.environ.get("CB200_GROUPED_GEMM", "native") == "native"
-            and torch.cuda.get_device_capability(x.device)[0] == 10)
+            and torch.cuda.get_device_capability(x.device)[0] == 9)
 
 
 def _padded_counts(counts: torch.Tensor) -> torch.Tensor:

@@ -1,6 +1,6 @@
 """Grouped (variable-M) linear: rows grouped by expert, one weight matrix per expert.
 
-CUDA path: our tcgen05 grouped GEMM (`kernel/csrc/grouped_gemm_tcgen05.cu`) - ONE persistent launch per GEMM walks a tile
+CUDA path: our wgmma grouped GEMM (`kernel/csrc/grouped_gemm_wgmma.cu`) - ONE persistent launch per GEMM walks a tile
 list built on the device from the per-expert row counts (no host sync, no per-expert launches, no padding for the
 forward / dgrad; the weight-gradient GEMM reduces over each expert's token rows and wants the row ranges aligned to the
 128-row k-block, which `_pad_groups` arranges on the device when the caller's layout is not aligned already).
@@ -33,7 +33,7 @@ def native_ok(x: torch.Tensor, w: torch.Tensor) -> bool:
         return False
     return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and w.dtype == x.dtype and x.dim() == 2
             and w.dim() == 3 and x.shape[0] > 0 and x.shape[1] % 8 == 0 and w.shape[1] % 8 == 0 and w.shape[0] <= 512
-            and w.is_contiguous() and torch.cuda.get_device_capability(x.device)[0] == 10)
+            and w.is_contiguous() and torch.cuda.get_device_capability(x.device)[0] == 9)
 
 
 def _offs(counts: torch.Tensor, device) -> torch.Tensor:

@@ -1,4 +1,4 @@
-"""FusedAdam: one multi-tensor launch per param group (sm_100a kernel; torch `_foreach` reference on CPU).
+"""FusedAdam: one multi-tensor launch per param group (sm_90a kernel; torch `_foreach` reference on CPU).
 Parity: reference `colossalai/nn/optimizer/fused_adam.py` (multi_tensor_adam, adamw_mode, div_scale)."""
 from __future__ import annotations
 

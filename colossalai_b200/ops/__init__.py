@@ -1,4 +1,4 @@
-"""Python face of the native op set.  CUDA tensors -> sm_100a kernels; CPU tensors -> PyTorch reference."""
+"""Python face of the native op set.  CUDA tensors -> sm_90a kernels; CPU tensors -> PyTorch reference."""
 from ._dispatch import force_torch, is_forced_torch, use_native
 from .activation import bias_act, get_activation, glu, glu_ref, swiglu
 from .attention import attention, attention_ref, attention_with_lse_ref

@@ -1,6 +1,6 @@
 """Native-vs-reference dispatch policy shared by every op.
 
-Rule: CUDA tensors -> the sm_100a kernel (hard error if its library is missing on a GPU box);
+Rule: CUDA tensors -> the sm_90a kernel (hard error if its library is missing on a GPU box);
 CPU tensors -> the plain PyTorch reference (CPU plumbing tier).  `CB200_FORCE_TORCH=1` forces the reference
 path on GPU too (used by the numerics tests and by the "baseline mode" of the benchmarks).
 """

@@ -1,7 +1,7 @@
 """Attention front-end on token-major (packed / varlen) tensors.
 
 q: [T, Hq, D]; k, v: [Tk, Hkv, D].  Sequences are either uniform (`batch` x `seqlen`) or described by
-`cu_seqlens` (packed).  Backends: `native` = our sm_100a flash-attention (kernel/csrc/flash_attn_tcgen05.cu),
+`cu_seqlens` (packed).  Backends: `native` = our sm_90a flash-attention (kernel/csrc/flash_attn_wgmma.cu),
 `torch` = SDPA reference (CPU tier, oracle).  Parity: reference `ColoAttention.attention`
 (`colossalai/shardformer/layer/attn.py:82-331`) and its FlashAttention*Loader dispatch.
 """

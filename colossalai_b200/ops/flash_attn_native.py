@@ -1,6 +1,5 @@
-"""ctypes face of the sm_100a flash-attention kernels (`kernel/csrc/flash_attn_tcgen05.cu`): tcgen05 forward (validated
-on a B200 in round 2: 17/17 numerics cases) and tcgen05 backward (dK / dV accumulated in TMEM per key tile over the whole
-GQA group, dQ through fp32 reductions).
+"""ctypes face of the sm_90a flash-attention kernels (`kernel/csrc/flash_attn_wgmma.cu`): wgmma forward and wgmma
+backward (dK / dV accumulated in registers per key tile over the whole GQA group, dQ through fp32 reductions).
 
 `CB200_FLASH_NATIVE=1` (or `enable(True)`) routes `ops.attention` and the ring-attention block functions through them
 for equal-length bf16 / fp16 batches (head_dim 64 / 128 forward, 128 backward; sequence length a multiple of 128);
@@ -48,7 +47,7 @@ def supported(q, k, v, cu_seqlens_q=None, cu_seqlens_k=None, force: bool = False
         return False
     if cu_seqlens_q is not None and cu_seqlens_k is not None and cu_seqlens_k is not cu_seqlens_q:
         return False
-    if not (_tensor_ok(q) and _tensor_ok(k) and _tensor_ok(v)) or torch.cuda.get_device_capability()[0] != 10:
+    if not (_tensor_ok(q) and _tensor_ok(k) and _tensor_ok(v)) or torch.cuda.get_device_capability()[0] != 9:
         return False
     D = q.shape[-1]
     return D in (64, 128) and k.shape[-1] == D and v.shape[-1] == D and q.shape[1] % k.shape[1] == 0 \

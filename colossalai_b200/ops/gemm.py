@@ -1,7 +1,7 @@
 """Dense GEMM entry points used by every linear layer.
 
 `linear_forward(x, w)` = x @ w^T, `matmul_nn(a, b)` = a @ b, `matmul_tn(a, b)` = a^T @ b (wgrad).
-Native path: our tcgen05/TMEM/TMA GEMM (kernel/csrc/gemm_tcgen05.cu) for bf16/fp16 on sm_100a when the shape is
+Native path: our wgmma/TMA GEMM (kernel/csrc/gemm_wgmma.cu) for bf16/fp16 on sm_90a when the shape is
 tile-aligned; otherwise cuBLAS through torch (plain library GEMM).  Parity: every `F.linear` / `torch.matmul`
 call site in the reference's `shardformer/layer/_operation.py:90-737`.
 """
@@ -16,8 +16,7 @@ import torch.nn.functional as F
 from ._dispatch import use_native
 
 _native = None
-# plain (un-fused) GEMMs: "cublas" = library GEMM through torch (default: the library's 2x2-cluster kernels are still
-# ~8 % ahead of our CTA-pair kernel, see profiles/gemm_tcgen05_2cta_vs_cublas_r1.jsonl), "native" = our tcgen05 kernel.
+# plain (un-fused) GEMMs: "cublas" = library GEMM through torch (default), "native" = our wgmma kernel.
 # The comm-fused GEMMs (parallel/fused.py) always run our main loop - there is no library equivalent.
 _BACKEND = os.environ.get("CB200_GEMM_BACKEND", "cublas")
 

@@ -1,4 +1,4 @@
-"""ctypes face of the tcgen05 GEMM (kernel/csrc/gemm_tcgen05.cu)."""
+"""ctypes face of the wgmma GEMM (kernel/csrc/gemm_wgmma.cu)."""
 from __future__ import annotations
 
 import ctypes
@@ -25,7 +25,7 @@ def _get_lib():
 def available() -> bool:
     if _DISABLED or not torch.cuda.is_available():
         return False
-    if torch.cuda.get_device_capability()[0] != 10:
+    if torch.cuda.get_device_capability()[0] != 9:
         return False
     try:
         _get_lib()
@@ -100,7 +100,7 @@ def gemm_tn(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None
 
 # ---- fp8: c[M,N] = scale_a * scale_b * (a[M,K] @ b[N,K]^T), operands e4m3 / e5m2, both K-major
 _FP8_FMT = {getattr(torch, "float8_e4m3fn", None): 0, getattr(torch, "float8_e5m2", None): 1}
-_FP8_BACKEND = os.environ.get("CB200_FP8_GEMM", "native")      # "native" -> CTA-pair tcgen05 kind::f8f6f4 kernel
+_FP8_BACKEND = os.environ.get("CB200_FP8_GEMM", "native")      # "native" -> wgmma m64n128k32 fp8 kernel
 
 
 def fp8_backend() -> str:
@@ -121,7 +121,10 @@ def supported_fp8_nt(a: torch.Tensor, b: torch.Tensor) -> bool:
     if not (a.is_cuda and ok(a) and ok(b) and a.shape[1] == b.shape[1]):
         return False
     M, K, N = a.shape[0], a.shape[1], b.shape[0]
-    return M >= 256 and N >= 256 and K >= 256 and N % 8 == 0 and ((M + 255) // 256) * ((N + 255) // 256) >= 37
+    # the kernel runs one persistent CTA per SM on 128 x 128 output tiles: shapes with fewer tiles than half the SMs
+    # would leave most of the GPU idle, and go to cuBLASLt instead
+    sms = torch.cuda.get_device_properties(a.device).multi_processor_count
+    return M >= 128 and N >= 128 and K >= 128 and N % 8 == 0 and ((M + 127) // 128) * ((N + 127) // 128) >= sms // 2
 
 
 def gemm_fp8_nt(a: torch.Tensor, b: torch.Tensor, scale_a: Optional[torch.Tensor], scale_b: Optional[torch.Tensor],

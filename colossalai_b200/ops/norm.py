@@ -1,6 +1,6 @@
 """Fused RMSNorm / LayerNorm (fwd + bwd, optional fused residual add).
 
-Native path: `kernel/csrc/norm.cu` (sm_100a).  Reference path (CPU tensors / CB200_FORCE_TORCH): plain PyTorch
+Native path: `kernel/csrc/norm.cu` (sm_90a).  Reference path (CPU tensors / CB200_FORCE_TORCH): plain PyTorch
 fp32 math.  Parity: reference apex FusedRMSNorm / FusedLayerNorm wrappers
 (`colossalai/shardformer/layer/normalization.py:27-135`) and `inference_ops.fused_add_rms_layernorm` (N17).
 """

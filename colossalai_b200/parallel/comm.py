@@ -1,8 +1,8 @@
 """Functional collectives on contiguous tensors (the NCCL/gloo baseline backend and correctness oracle).
 
 Every comm-bound op in the framework has two interchangeable backends behind one autograd Function:
-this module (`torch.distributed`: NCCL on B200, gloo on the CPU plumbing tier, also the multi-node path) and
-`colossalai_b200.parallel.fused` (sm_100a kernels over NVLink peer memory).  Parity: the raw collective call
+this module (`torch.distributed`: NCCL on the GPU, gloo on the CPU plumbing tier, also the multi-node path) and
+`colossalai_b200.parallel.fused` (sm_90a kernels over NVLink peer memory).  Parity: the raw collective call
 sites inventoried in SURVEY §2.12 (`shardformer/layer/_operation.py:1187-1282`).
 """
 from __future__ import annotations

@@ -114,21 +114,15 @@ class FusedWorkspace:
         self.rank = comm.group_rank(group)
         lib = _get_lib()
         self.flags = _SymmBuffer(4 * lib.cb_fused_flag_words(), self.group, zero=True)
-        # tile-granular GEMM->RS pipeline: symmetric epoch flags [16 writer ranks][tile_flag_stride]
-        self.tile_flag_stride = 8192
-        self.tile_flags = _SymmBuffer(4 * 16 * self.tile_flag_stride, self.group, zero=True)
         torch.cuda.synchronize()
         dist.barrier(group=self.group)      # flag pages are zero everywhere before first use
         self.epoch = 0
         self._in: Dict[int, List[_SymmBuffer]] = {}
         self._part: Dict[int, List[_SymmBuffer]] = {}
-        self._ar: Dict[int, List[_SymmBuffer]] = {}
         self._toggle: Dict[Tuple[str, int], int] = {}
         self._counters: Dict[int, torch.Tensor] = {}
         dev = torch.device("cuda", torch.cuda.current_device())
         self.chunk_counter = torch.zeros(64, dtype=torch.int32, device=dev)
-        self.tile_counter = torch.zeros(1 << 16, dtype=torch.int32, device=dev)
-        self.rs_progress = torch.zeros(1 << 17, dtype=torch.int32, device=dev)
 
     def next_epoch(self) -> int:
         self.epoch += 1
@@ -265,7 +259,6 @@ def all_gather_gemm(x_local: torch.Tensor, w: torch.Tensor, group: Optional[Proc
 
 
 # ------------------------------------------------------------------------------------------------ GEMM + RS
-_RS_VARIANTS = {"auto": 0, "stagger": 1, "stream": 2}
 _rs_choice: Dict[Tuple, str] = {}            # autotuned variant per (world, T, N, K, layout, dtype)
 rs_tuning_log: List[dict] = []               # what the autotuner measured (bench.py / profiles print it)
 
@@ -280,38 +273,24 @@ def _gemm_rs_lib(a, w, group, transpose_b):
     return comm.reduce_scatter(full, 0, group)
 
 
-def _gemm_rs_launch(ws, a, w, transpose_b, block_n, variant: str, ar_out: Optional["_SymmBuffer"] = None):
+def _gemm_rs_launch(ws, a, w, transpose_b, block_n):
     lib = _get_lib()
     T, K = a.shape
     N = w.shape[0] if transpose_b else w.shape[1]
     world = ws.world
     part = ws.part_buffer(T * N * a.element_size())
     epoch = ws.next_epoch()
-    out = None if ar_out is not None else torch.empty(T // world, N, dtype=a.dtype, device=a.device)
+    out = torch.empty(T // world, N, dtype=a.dtype, device=a.device)
     mc = ctypes.c_void_p(part.mc_ptr) if (part.mc_ptr and a.dtype == torch.bfloat16
                                           and os.environ.get("CB200_NO_MULTIMEM", "0") != "1") else ctypes.c_void_p(0)
     loader.check(lib.cb_gemm_rs(loader.ptr(a), loader.ptr(w), ctypes.c_void_p(part.peer_ptrs[ws.rank]),
                                 part.ptr_array(world), mc, ws.flags.ptr_array(world), loader.ptr(ws.chunk_counter),
-                                loader.ptr(out) if out is not None else ctypes.c_void_p(0), T, N, K, a.stride(0),
+                                loader.ptr(out), T, N, K, a.stride(0),
                                 w.stride(0), N, 0,
                                 0 if transpose_b else 1, code(a.dtype), ws.rank, world, ctypes.c_uint32(epoch), block_n,
-                                ws.tile_flags.ptr_array(world), ws.tile_flag_stride, loader.ptr(ws.tile_counter),
-                                ws.tile_counter.numel(), loader.ptr(ws.rs_progress), ws.rs_progress.numel(),
-                                _RS_VARIANTS[variant], ctypes.c_void_p(ar_out.mc_ptr if ar_out is not None else 0),
                                 loader.stream_ptr()), "gemm_rs")
     part.last_epoch = epoch
-    if ar_out is not None:
-        ar_out.last_epoch = 0          # the kernel itself waited until every rank's broadcast landed
     return out
-
-
-def _stream_capable(ws, a, T, N, world) -> bool:
-    """The streamed in-switch reduction needs the NVLS multicast mapping, bf16 partials and whole 256 x 256 tiles."""
-    if a.dtype != torch.bfloat16 or N % 256 != 0 or (T // world) % 256 != 0:
-        return False
-    if os.environ.get("CB200_NO_MULTIMEM", "0") == "1":
-        return False
-    return bool(ws.flags.mc_ptr)
 
 
 def _time_rs(fn, group, iters: int = 3) -> float:
@@ -331,9 +310,10 @@ def _time_rs(fn, group, iters: int = 3) -> float:
 
 
 def rs_variant(a: torch.Tensor, w: torch.Tensor, group: Optional[ProcessGroup], transpose_b: bool = True) -> str:
-    """Which implementation `gemm_reduce_scatter` uses for this shape: 'stream' (tcgen05 GEMM + in-switch
-    `multimem.ld_reduce` of finished tiles), 'stagger' (tcgen05 GEMM + staggered P2P pull-accumulate), or 'lib'
-    (cuBLAS/own GEMM followed by the NCCL reduce-scatter).  Chosen ONCE per shape by measuring all candidates on the
+    """Which implementation `gemm_reduce_scatter` uses for this shape: 'fused' (one kernel: the wgmma GEMM writes
+    partial tiles to symmetric memory, then every rank reduces its own chunk - in the switch with `multimem.ld_reduce`
+    when a multicast mapping exists, else with P2P loads - once all peers have finished that chunk; the reduction
+    does not overlap the GEMM), or 'lib' (cuBLAS/own GEMM followed by the NCCL reduce-scatter).  Chosen ONCE per shape by measuring all candidates on the
     live tensors (device-timed, max over ranks, identical decision on every rank); `CB200_FUSED_RS` forces one."""
     ws = workspace(group)
     T, K = a.shape
@@ -342,20 +322,19 @@ def rs_variant(a: torch.Tensor, w: torch.Tensor, group: Optional[ProcessGroup], 
     if not _rs_fusable(ws, a, w, T, K, N, world):
         return "lib"
     forced = os.environ.get("CB200_FUSED_RS", "auto")
-    can_stream = _stream_capable(ws, a, T, N, world)
-    if forced in ("stagger", "lib") or (forced == "stream" and can_stream):
+    if forced in ("fused", "lib"):
         return forced
     key = (world, T, N, K, transpose_b, a.dtype)
     got = _rs_choice.get(key)
     if got is not None:
         return got
-    cands = ["stagger"] + (["stream"] if can_stream else []) + ["lib"]
+    cands = ["fused", "lib"]
     times = {}
     for c in cands:
         if c == "lib":
             times[c] = _time_rs(lambda: _gemm_rs_lib(a, w, group, transpose_b), ws.group)
         else:
-            times[c] = _time_rs(lambda c=c: _gemm_rs_launch(ws, a, w, transpose_b, 0, c), ws.group)
+            times[c] = _time_rs(lambda: _gemm_rs_launch(ws, a, w, transpose_b, 0), ws.group)
     # prefer our own kernels on a tie (2 %): the library path is the fallback, not the product
     best = min(cands, key=lambda c: times[c] * (1.02 if c == "lib" else 1.0))
     _rs_choice[key] = best
@@ -368,8 +347,10 @@ def gemm_reduce_scatter(a: torch.Tensor, w: torch.Tensor, group: Optional[Proces
                         block_n: int = 0, variant: str = "auto") -> torch.Tensor:
     """out[T/world, N] = reduce_scatter_rows(a @ (w^T if transpose_b else w)).
 
-    variant: 'auto' = the autotuned choice of `rs_variant`; 'stagger' / 'stream' force one fused kernel; 'lib' = GEMM +
-    NCCL reduce-scatter."""
+    variant: 'auto' = the autotuned choice of `rs_variant`; 'fused' forces the fused kernel; 'lib' = GEMM + NCCL
+    reduce-scatter."""
+    if variant not in ("auto", "fused", "lib"):
+        raise ValueError(f"unknown GEMM->reduce-scatter variant {variant!r} (auto / fused / lib)")
     ws = workspace(group)
     T, K = a.shape
     N = w.shape[0] if transpose_b else w.shape[1]
@@ -380,13 +361,11 @@ def gemm_reduce_scatter(a: torch.Tensor, w: torch.Tensor, group: Optional[Proces
     if variant == "auto" and block_n == 0:
         variant = rs_variant(a, w, group, transpose_b)
     elif variant == "auto":
-        variant = "stagger"
+        variant = "fused"
     if variant == "lib":
         stats["rs_lib"] = stats.get("rs_lib", 0) + 1
         return _gemm_rs_lib(a, w, group, transpose_b)
-    if variant == "stream" and not _stream_capable(ws, a, T, N, world):
-        variant = "stagger"
-    out = _gemm_rs_launch(ws, a, w, transpose_b, block_n, variant)
+    out = _gemm_rs_launch(ws, a, w, transpose_b, block_n)
     loader.launch_counter.add("fused_gemm_rs")
     stats["gemm_rs"] += 1
     stats["rs_" + variant] = stats.get("rs_" + variant, 0) + 1
@@ -395,11 +374,9 @@ def gemm_reduce_scatter(a: torch.Tensor, w: torch.Tensor, group: Optional[Proces
 
 # ------------------------------------------------------------------------------------------------ GEMM + AR
 def gemm_all_reduce(a: torch.Tensor, w: torch.Tensor, group: Optional[ProcessGroup]) -> torch.Tensor:
-    """all_reduce(a @ w^T) in ONE kernel: every rank runs the tcgen05 GEMM into its symmetric partial buffer; the owner
-    of a row chunk reduces each finished tile inside the NVSwitch (`multimem.ld_reduce`) and broadcasts the result to
-    all ranks through the multicast mapping of the output (`multimem.st`) - the row-linear forward of tensor
-    parallelism without sequence parallelism (reference: `F.linear` + `dist.all_reduce`, `layer/linear.py:586-587`).
-    Shapes the streamed kernel does not take fall back to fused reduce-scatter + NVLink pull all-gather."""
+    """all_reduce(a @ w^T) as the fused GEMM->reduce-scatter followed by the NVLink pull all-gather - the row-linear
+    forward of tensor parallelism without sequence parallelism (reference: `F.linear` + `dist.all_reduce`,
+    `layer/linear.py:586-587`)."""
     ws = workspace(group)
     world = comm.group_size(group)
     T, K = a.shape
@@ -409,15 +386,6 @@ def gemm_all_reduce(a: torch.Tensor, w: torch.Tensor, group: Optional[ProcessGro
         y = torch.nn.functional.linear(a, w)
         comm.all_reduce(y, group)
         return y
-    if _stream_capable(ws, a, T, N, world) and os.environ.get("CB200_FUSED_AR", "multimem") == "multimem":
-        nbytes = T * N * a.element_size()
-        out_buf = ws._pool(ws._ar, "ar", nbytes)
-        if out_buf.mc_ptr:
-            _gemm_rs_launch(ws, a, w, True, 0, "stream", ar_out=out_buf)
-            loader.launch_counter.add("fused_gemm_ar")
-            stats["gemm_ar"] = stats.get("gemm_ar", 0) + 1
-            # hand out a private copy: the symmetric buffer is reused by the call after next
-            return out_buf.tensor[:nbytes].view(a.dtype).view(T, N).clone()
     return all_gather(gemm_reduce_scatter(a, w, group, transpose_b=True), group)
 
 

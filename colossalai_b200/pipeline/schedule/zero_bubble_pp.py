@@ -2,7 +2,7 @@
 
 Parity: reference `colossalai/pipeline/schedule/zero_bubble_pp.py:40-971` (`ZeroBubbleVPipeScheduler`: iterate a
 precomputed list of `ScheduledNode{F,B,W,SEND_*,RECV_*}`; B computes dX only, W pops the `WeightGradStore`).
-Communication design differs (B200/NCCL-first): every adjacent stage pair gets TWO dedicated 2-rank process groups, one
+Communication design differs (NCCL-first): every adjacent stage pair gets TWO dedicated 2-rank process groups, one
 per direction, so opposite-direction traffic never shares a NCCL stream (no send/recv cross dead-lock, no need to
 coalesce ops); all sends are asynchronous; receives on a channel are posted in the SENDER's order (known from the global
 schedule), a bounded number of messages ahead of their consumer.

@@ -4,9 +4,9 @@ Parity: reference `colossalai/quantization/fp8.py` (cast_to_fp8:51, cast_from_fp
 all_to_all_single_fp8:258, cast_{to,from}_fp8_pipeline:285/327, reduce_scatter_fp8:401, DDP/FSDP hooks:408-600,
 all_to_all_fp8:648, all_gather_fp8:680, linear_fp8:842).
 
-B200 design: the amax reduction + scaled cast run as native kernels (kernel/csrc/quant.cu), payloads travel as raw bytes
+Design: the amax reduction + scaled cast run as native kernels (kernel/csrc/quant.cu), payloads travel as raw bytes
 (`uint8` views) so the same code drives NCCL and gloo; the FP8 matmul is cuBLASLt's scaled GEMM (`torch._scaled_mm`) or, with
-`CB200_FP8_GEMM=native`, the hand-written CTA-pair tcgen05 `kind::f8f6f4` kernel (kernel/csrc/gemm_tcgen05.cu).
+`CB200_FP8_GEMM=native`, the hand-written wgmma fp8 kernel (kernel/csrc/gemm_wgmma.cu).
 """
 from __future__ import annotations
 

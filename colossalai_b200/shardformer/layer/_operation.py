@@ -4,9 +4,9 @@ Parity: reference `colossalai/shardformer/layer/_operation.py:76-1393`
 (`LinearWithAsyncCommunication`, `_LinearWithGatherForwardReduceScatterBackward`,
 `_LinearWithReduceScatterForwardGatherBackward`, `_AllToAll`, split/gather/reduce fwd-bwd pairs, ring variants).
 
-B200-first design: each comm-bound linear is ONE autograd Function with two interchangeable backends —
+H100-first design: each comm-bound linear is ONE autograd Function with two interchangeable backends —
 `nccl` (torch.distributed collectives + GEMM; also the gloo CPU tier and the correctness oracle) and `fused`
-(`colossalai_b200.parallel.fused`: a single sm_100a kernel that overlaps the tcgen05 GEMM tiles with P2P /
+(`colossalai_b200.parallel.fused`: a single sm_90a kernel that overlaps the wgmma GEMM tiles with P2P /
 multimem traffic over NVLink).  Weight-gradient GEMMs can be deferred (`WeightGradStore`) for zero-bubble PP.
 """
 from __future__ import annotations
@@ -37,7 +37,7 @@ _SAVE_GATHERED = os.environ.get("CB200_SP_SAVE_GATHERED", "1") != "0"
 
 
 def set_comm_backend(name: str) -> None:
-    """'nccl' (torch.distributed) or 'fused' (sm_100a fused compute+collective kernels over peer memory)."""
+    """'nccl' (torch.distributed) or 'fused' (sm_90a fused compute+collective kernels over peer memory)."""
     global _COMM_BACKEND
     assert name in ("nccl", "fused")
     _COMM_BACKEND = name
@@ -56,8 +56,9 @@ def _use_fused(x: torch.Tensor, group) -> bool:
 
 
 def _fused_rs_variant(a: torch.Tensor, weight: torch.Tensor, group, transpose_b: bool) -> str:
-    """Implementation of GEMM->reduce-scatter for this shape: 'stream' / 'stagger' (one fused sm_100a kernel) or 'lib'
-    (GEMM + NCCL reduce-scatter).  Measured once per shape on the live tensors by `parallel.fused.rs_variant` - round 1
+    """Implementation of GEMM->reduce-scatter for this shape: 'fused' (one sm_90a kernel: GEMM, then the reduction of
+    this rank's chunk) or 'lib' (GEMM + NCCL reduce-scatter).  Measured once per shape on the live tensors by
+    `parallel.fused.rs_variant` - round 1
     used a fixed reduction-depth threshold (K >= 2048) taken from the TP=8 timings, which was wrong at other TP
     degrees and froze the library fallback in place."""
     from ...parallel import fused

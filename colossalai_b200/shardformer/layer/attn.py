@@ -2,7 +2,7 @@
 
 Parity: reference `colossalai/shardformer/layer/attn.py:82-331` (ColoAttention.prepare_attn_kwargs / attention)
 and `:406-1247` (RingAttention: zigzag ring, online-softmax merge, dKV ring in backward, varlen).
-B200-first: tensors are token-major `[T, H, D]`; on one NVSwitch box every peer is one hop, so the "double ring"
+H100-first: tensors are token-major `[T, H, D]`; on one NVSwitch box every peer is one hop, so the "double ring"
 topology heuristics are dropped; KV (only the H_kv GQA heads, never repeat_kv'ed) is fetched from the owner rank —
 through NCCL P2P on the baseline backend, straight from peer HBM inside the attention kernel on the fused backend.
 """
@@ -110,7 +110,7 @@ def _lib_flash_ok(q: torch.Tensor) -> bool:
 
 def _block_fwd(q, k, v, batch, causal, scale):
     """One attention block returning (out [T,Hq,D], lse [T,Hq] fp32).  CUDA: the library flash kernel through aten (it
-    returns the log-sum-exp needed by the online-softmax merge) until the tcgen05 kernel lands; CPU: explicit softmax."""
+    returns the log-sum-exp needed by the online-softmax merge) until the wgmma kernel lands; CPU: explicit softmax."""
     from ...ops import flash_attn_native as fa
 
     if q.is_cuda and fa.supported(q, k, v, None):
@@ -389,7 +389,7 @@ class RingAttention(torch.autograd.Function):
         from . import ring_attn_fused as rf
 
         if rf.available(q, k, sp_group, batch):
-            # sm_100a path: KV tiles are TMA-loaded from the owner's HBM inside the attention main loop, the softmax
+            # sm_90a path: KV tiles are TMA-loaded from the owner's HBM inside the attention main loop, the softmax
             # state is merged in registers, dK / dV are reduced into the owner's accumulators (ring_attn_fused.py)
             return rf.ring_attention_fused(q, k, v, sp_group, batch, scale)
         return RingAttention.apply(q, k, v, sp_group, batch, scale)

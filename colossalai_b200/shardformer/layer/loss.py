@@ -2,7 +2,7 @@
 
 Parity: reference `colossalai/shardformer/layer/loss.py:25-356` (`DistCrossEntropy`, `DistLogProb`,
 `dist_cross_entropy` with label shift + SP/ring-attn label split + loss reduction over SP).
-B200-first: the three all-reduces of the reference (max, target-logit, exp-sum) are packed into two
+H100-first: the three all-reduces of the reference (max, target-logit, exp-sum) are packed into two
 (one MAX, one SUM over a stacked [2, T] buffer) and the softmax statistics / gradient come from a fused kernel
 (`ops.cross_entropy`), so the [T, V/tp] logits are read once in forward and written once in backward.
 """

@@ -1,4 +1,4 @@
-"""Norm layers backed by the fused sm_100a kernels (`ops.rms_norm`, `ops.layer_norm`).
+"""Norm layers backed by the fused sm_90a kernels (`ops.rms_norm`, `ops.layer_norm`).
 
 Parity: reference `colossalai/shardformer/layer/normalization.py:27-353` (`FusedRMSNorm`, `FusedLayerNorm`,
 `RMSNorm`, `LayerNorm` wrappers with `sp_partial_derived` marking).  No apex: the kernels are ours.

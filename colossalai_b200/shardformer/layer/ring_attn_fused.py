@@ -4,7 +4,7 @@ Reference being replaced: `RingAttention` in `colossalai/shardformer/layer/attn.
 flash-attn-2 calls with NCCL `batch_isend_irecv` of the (head-expanded) KV per hop, an elementwise `_rescale_out_lse`
 pass per hop on a second stream, and fp32 dKV buffers circulating around the ring in backward.
 
-B200-first design (one NVSwitch domain: every peer is one hop away at full bandwidth):
+H100-first design (one NVSwitch domain: every peer is one hop away at full bandwidth):
 
   * every rank PUBLISHES its K / V once per layer (GQA heads only) in a symmetric buffer; nobody forwards anything;
   * BACKWARD: the kernel of rank r reads the key / value tiles of block `src` STRAIGHT FROM RANK `src`'s HBM - its TMA

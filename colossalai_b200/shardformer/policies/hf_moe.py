@@ -7,7 +7,7 @@ That is exactly the contract of this framework's MoE data path, so the policy
   * keeps only the LOCAL experts' slices of the two parameters on every rank of `shard_config.ep_group`
     (parameter replacement; the slices are tagged so that checkpoints gather them), and
   * rebinds `MixtralExperts.forward` to `moe.dispatch_combine.moe_forward`: dropless dispatch to the owners (fused
-    NVLink dispatch on sm_100a, uneven all-to-all elsewhere), grouped per-expert GEMMs on the local slices, SwiGLU,
+    NVLink dispatch on sm_90a, uneven all-to-all elsewhere), grouped per-expert GEMMs on the local slices, SwiGLU,
     combine with the routing weights;
 the router (`gate`) stays replicated.  Attention is tensor-parallel like the llama-likes when TP is enabled.  Expert
 gradients are already sums over every token of the expert-parallel group that chose the expert; the usual 1 / ep scaling

@@ -1,6 +1,6 @@
 """ShardConfig: the one dataclass that carries parallel groups and feature flags to policies and layers.
 
-Parity: reference `colossalai/shardformer/shard/shard_config.py:13-130`.  B200 additions: `comm_backend`
+Parity: reference `colossalai/shardformer/shard/shard_config.py:13-130`.  Additions: `comm_backend`
 ("nccl" | "fused") selects the fused compute+collective kernels, `seq_dim` is the token dim of activations
 (token-major models use 0).
 """
@@ -42,7 +42,7 @@ class ShardConfig:
     sp_axis: Optional[int] = None
     pg_mesh: Optional[Any] = None
     inner_ring_size: Optional[int] = None
-    # B200-native knobs
+    # H100-native knobs
     comm_backend: str = "nccl"
     seq_dim: int = 0
     use_zbv: bool = False

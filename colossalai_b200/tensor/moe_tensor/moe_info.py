@@ -9,7 +9,7 @@ __all__ = ["MoeParallelInfo"]
 
 
 class MoeParallelInfo:
-    """Ranks are laid out `[pp, dp, ep]` (`ep_inside=True`, expert-parallel ranks adjacent — one NVSwitch hop on B200
+    """Ranks are laid out `[pp, dp, ep]` (`ep_inside=True`, expert-parallel ranks adjacent — one NVSwitch hop
     either way) or `[pp, ep, dp]`.  Holds the EP / DP group of the calling rank and their rank lists."""
 
     def __init__(self, ep_inside: bool, ep_size: int, dp_size: int, pp_size: int = 1) -> None:

@@ -1,5 +1,5 @@
 """Device-synchronising timers.  Parity: reference `colossalai/utils/timer.py:9,91`.  `CudaEventTimer` is the
-B200 addition: device-side timing with CUDA events (what every reported number must use)."""
+Addition: device-side timing with CUDA events (what every reported number must use)."""
 from __future__ import annotations
 
 import time

@@ -3,7 +3,7 @@
 Parity: reference `colossalai/zero/gemini/gemini_optimizer.py:70-874`: optimizer params are views into the fp32 master
 shard of each chunk (per original parameter, so per-group hyper-parameters keep working); gradients come from the
 reduced gradient shards; loss-scale / overflow / clipping use chunk l2 norms reduced over the zero (and tp) group;
-`HybridAdam` runs the AVX-512 kernel on host-resident shards and the multi-tensor sm_100a kernel on device-resident
+`HybridAdam` runs the AVX-512 kernel on host-resident shards and the multi-tensor sm_90a kernel on device-resident
 ones; afterwards the low-precision working shards are refreshed from the master shards.
 """
 from __future__ import annotations

@@ -6,7 +6,7 @@ ZeRO-1 (grads kept until the sync point, `no_sync` accumulation) vs ZeRO-2 (redu
 complete and free the full bucket), unscale + clip with hybrid-aware norm, updated working params all-gathered,
 several dp groups (`pg_to_param_list`, used for MoE expert params), cpu_offload of master/optimizer states.
 
-B200-first layout: the working parameters of a bucket are *views of one flat buffer*; every rank owns a contiguous 1/dp
+H100-first layout: the working parameters of a bucket are *views of one flat buffer*; every rank owns a contiguous 1/dp
 slice of each bucket.  So a bucket needs exactly one `reduce_scatter_tensor` (grads) and one `all_gather_into_tensor`
 (updated params) with no flatten / unflatten copies, and the fused Adam kernel updates master shard + moments and writes
 the low-precision slice in one launch.

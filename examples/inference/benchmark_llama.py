@@ -71,7 +71,7 @@ def main():
            "our_kernel_launches": loader.launch_counter.count,
            "peak_mem_gib": torch.cuda.max_memory_allocated() / 2**30}
     # decode is HBM-bound: every step streams all weights once plus the live KV cache; roofline = bytes / measured
-    # copy bandwidth (MEASURED_PEAKS.json, 6555.8 GB/s on this pool's B200s)
+    # copy bandwidth (MEASURED_PEAKS.json when present)
     hbm_gbs = 6555.8
     try:
         hbm_gbs = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..",

@@ -1,7 +1,7 @@
 """Long-context training with zigzag ring attention (context parallelism): every rank holds 1 / sp of the sequence,
-attention runs blockwise against the K/V of all ranks (fused NVLink path on sm_100a, python ring elsewhere), everything
-else is sequence-local.  BASELINE config 5 is `--model llama3-8b --seq 131072 --sp 8 --zero 1 --grad-ckpt` on 8 x B200
-(5.4 s / step, `profiles/llama3_8b_128k_sp8_ring_r2.log`).
+attention runs blockwise against the K/V of all ranks (fused NVLink path on sm_90a, python ring elsewhere), everything
+else is sequence-local.  BASELINE config 5 is `--model llama3-8b --seq 131072 --sp 8 --zero 1 --grad-ckpt` on 8 GPUs
+(not measured on H100).
 
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 examples/language/long_context/train_ring_attention.py \\
         --model llama3-8b --seq 131072 --sp 8 --zero 1 --grad-ckpt

@@ -3,7 +3,7 @@ examples/language/mixtral/benchmark.py and examples/language/deepseek/benchmark.
 
     torchrun --nproc-per-node 8 examples/language/mixtral/benchmark.py -c mixtral-8x7b --layers 4 --ep 8 --zero 1 -b 2 -l 4096
 
-Prints device-timed tokens/s (max over ranks), the MoE back ends in use (fused NVLink dispatch/combine + tcgen05 grouped
+Prints device-timed tokens/s (max over ranks), the MoE back ends in use (fused NVLink dispatch/combine + wgmma grouped
 GEMM vs NCCL all-to-all + library grouped GEMM: `--moe_backend`, `--grouped_gemm`) and peak memory.  `--layers` cuts the
 depth so the full-width model fits one box without pipeline stages (Mixtral-8x7B is 47 B parameters); the per-layer
 expert shapes - which is what the EP kernels see - are unchanged.

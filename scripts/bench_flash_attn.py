@@ -1,4 +1,4 @@
-"""tcgen05 flash-attention forward vs the library SDPA (cuDNN / flash) on the Llama-3-8B attention shape."""
+"""wgmma flash-attention forward vs the library SDPA (cuDNN / flash) on the Llama-3-8B attention shape."""
 import json
 
 import torch
@@ -30,7 +30,7 @@ for (B, S, Hq, Hkv, D) in [(1, 4096, 32, 8, 128), (4, 4096, 32, 8, 128), (1, 163
     fl = 4.0 * B * Hq * S * S * D / 2
     print("FLASH_FWD " + json.dumps({"B": B, "S": S, "Hq": Hq, "Hkv": Hkv, "D": D, "native_ms": t_nat, "sdpa_ms": t_lib,
                                      "native_tflops": fl / t_nat / 1e9, "sdpa_tflops": fl / t_lib / 1e9}), flush=True)
-    # backward: ours = one launch chain (delta, tcgen05 bwd, dq cast); library = autograd through SDPA (cuDNN bprop)
+    # backward: ours = one launch chain (delta, wgmma bwd, dq cast); library = autograd through SDPA (cuDNN bprop)
     out, lse = fa.flash_fwd(q, k, v, B, True, None)
     dout = torch.randn_like(out)
     t_nat_b = timeit(lambda: fa.flash_bwd(q, k, v, out, dout, lse, B, True, None))

@@ -1,4 +1,4 @@
-"""fp8 tcgen05 GEMM vs cuBLASLt `_scaled_mm` vs bf16 cuBLAS on the Llama-3-8B forward shapes (CUDA events, L2 flushed
+"""fp8 wgmma GEMM vs cuBLASLt `_scaled_mm` vs bf16 cuBLAS on the Llama-3-8B forward shapes (CUDA events, L2 flushed
 by cycling through distinct operand buffers)."""
 import json
 

@@ -1,4 +1,4 @@
-"""Grouped expert GEMMs: our tcgen05 kernel vs the library `torch._grouped_mm` vs a per-expert cuBLAS loop, on the
+"""Grouped expert GEMMs: our wgmma kernel vs the library `torch._grouped_mm` vs a per-expert cuBLAS loop, on the
 expert-MLP shapes of Mixtral-8x7B and a DeepSeekMoE-16B-class layer (tokens per rank 8192, balanced routing)."""
 import json
 import os

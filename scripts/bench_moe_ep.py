@@ -1,4 +1,4 @@
-"""Expert-parallel MoE layer, device-timed (max over ranks): fused NVLink dispatch/combine + tcgen05 grouped GEMM vs the
+"""Expert-parallel MoE layer, device-timed (max over ranks): fused NVLink dispatch/combine + wgmma grouped GEMM vs the
 NCCL all-to-all composition (+ library grouped GEMM), forward + backward, 8192 tokens per rank.
 
     python -m torch.distributed.run --nproc-per-node N scripts/bench_moe_ep.py      (BASELINE.json config 4)

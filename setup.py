@@ -1,6 +1,6 @@
 """Editable install is optional: tests/bench add the repo root to sys.path themselves.
 `python setup.py build_ext --inplace` (or `python -m colossalai_b200.kernel.build`) compiles every native library
-for sm_100a into colossalai_b200/kernel/_build/."""
+for sm_90a into colossalai_b200/kernel/_build/."""
 from setuptools import find_packages, setup
 from setuptools.command.build_ext import build_ext as _build_ext
 

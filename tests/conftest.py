@@ -8,7 +8,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "dist: spawns multiple processes (gloo on CPU, NCCL on GPU)")
 
 

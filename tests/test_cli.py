@@ -11,7 +11,7 @@ from colossalai_b200.cli.launcher.run import fetch_hostfile, get_launch_command,
 def test_check_report(capsys):
     assert cli(["check", "-i"]) == 0
     out = capsys.readouterr().out
-    assert "Installation Report" in out and "sm_100a" in out
+    assert "Installation Report" in out and "sm_90a" in out
 
 
 def test_launch_command_and_hostfile():

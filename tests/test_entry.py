@@ -15,7 +15,7 @@ def test_smoke_runs_native_kernels():
 
 
 def test_extension_registry():
-    """Every reference extension name resolves to an in-tree sm_100a library descriptor (reference: extensions/)."""
+    """Every reference extension name resolves to an in-tree sm_90a library descriptor (reference: extensions/)."""
     from colossalai_b200.extensions import ALL_EXTENSIONS, CppExtension, CudaExtension, get_extension
 
     for name in ("cpu_adam_x86", "fused_optim_cuda", "layernorm_cuda", "moe_cuda", "scaled_masked_softmax_cuda",

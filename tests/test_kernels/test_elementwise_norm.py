@@ -1,4 +1,4 @@
-"""Numerics of the sm_100a norm / activation / rope / CE kernels against plain PyTorch fp32 references."""
+"""Numerics of the sm_90a norm / activation / rope / CE kernels against plain PyTorch fp32 references."""
 import pytest
 import torch
 

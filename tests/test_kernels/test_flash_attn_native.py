@@ -1,5 +1,4 @@
-"""tcgen05 flash-attention forward against an fp32 PyTorch reference (out and log-sum-exp), plus gradients.
-First hardware run (round 2): 17/17 pass on a B200 (gpurun_out/c1_flash_test.log)."""
+"""wgmma flash-attention forward against an fp32 PyTorch reference (out and log-sum-exp), plus gradients."""
 import os
 
 import pytest
@@ -53,7 +52,7 @@ def test_flash_native_gradients_match_library():
 @pytest.mark.parametrize("causal", [True, False])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_flash_bwd_matches_reference(B, S, Hq, Hkv, causal, dtype):
-    """tcgen05 backward (dq, dk, dv) against autograd through the explicit fp32 softmax reference."""
+    """wgmma backward (dq, dk, dv) against autograd through the explicit fp32 softmax reference."""
     from colossalai_b200.ops import flash_attn_native as fa
     from colossalai_b200.ops.attention import attention_with_lse_ref
 

@@ -1,4 +1,4 @@
-"""fp8 (E4M3 / E5M2) CTA-pair tcgen05 GEMM (`kind::f8f6f4`) against an fp32 PyTorch reference of the same
+"""fp8 (E4M3 / E5M2) wgmma GEMM (m64n128k32, fp32 promotion per 128-deep stage) against an fp32 PyTorch reference of the same
 de-quantised operands."""
 import os
 
@@ -23,7 +23,7 @@ def test_fp8_gemm_matches_fp32_reference(M, N, K, a_dtype, out_dtype):
     from colossalai_b200.ops import gemm_native
 
     if not gemm_native.available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     torch.manual_seed(0)
     adt = torch.float8_e4m3fn if a_dtype == "e4m3" else torch.float8_e5m2
     a, sa = _quant(torch.randn(M, K, device="cuda"), adt)
@@ -42,7 +42,7 @@ def test_linear_fp8_native_backend_matches_cublaslt():
     from colossalai_b200.quantization.fp8 import linear_fp8
 
     if not gemm_native.available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     torch.manual_seed(0)
     x = torch.randn(4096, 4096, device="cuda", dtype=torch.bfloat16, requires_grad=True)
     w = (torch.randn(6144, 4096, device="cuda", dtype=torch.bfloat16) * 0.02).requires_grad_()

@@ -1,5 +1,5 @@
-"""tcgen05 GEMM numerics vs fp32 torch.matmul for the three linear-layer GEMM flavours (NT / NN / TN), tails,
-accumulate-into-C and both tile widths."""
+"""wgmma GEMM numerics vs fp32 torch.matmul for the three linear-layer GEMM flavours (NT / NN / TN), tails and
+accumulate-into-C."""
 import pytest
 import torch
 

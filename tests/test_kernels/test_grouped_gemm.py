@@ -1,4 +1,4 @@
-"""tcgen05 grouped (per-expert) GEMM: forward / dgrad with variable rows per expert and wgrad with variable reduction
+"""wgmma grouped (per-expert) GEMM: forward / dgrad with variable rows per expert and wgrad with variable reduction
 length, against fp32 per-expert matmuls.  Expert sizes include 0, 1, non-multiples of the tile and of the k-block."""
 import pytest
 import torch

@@ -60,7 +60,7 @@ def _gpu_worker(rank, world_size, port):
     from colossalai_b200.shardformer.layer import ring_attn_fused as rf
 
     tol = dict(rtol=3e-2, atol=3e-2)
-    # fused ring attention (default on sm_100a): KV tiles TMA-loaded from the owner's HBM inside the kernel, in-kernel
+    # fused ring attention (default on sm_90a): KV tiles TMA-loaded from the owner's HBM inside the kernel, in-kernel
     # softmax-state merge, dK / dV reduced into the owner's accumulators.  GQA, batch > 1, repeated layers (buffer reuse)
     for (B, S, Hq, Hkv) in [(2, 1024, 8, 2), (1, 2048 * world_size, 8, 2), (1, 512, 4, 4)]:
         for _ in range(2):
