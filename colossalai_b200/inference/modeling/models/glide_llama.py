@@ -16,6 +16,7 @@ import torch.nn.functional as F
 
 from ....models.config import ModelConfig
 from ....models.transformer import DecoderLayer, TransformerLMHeadModel, build_norm
+from ....ops.inference import gather_paged_kv
 from ...spec.struct import GlideInput
 
 __all__ = ["GlideLlamaConfig", "LlamaCrossAttention", "GlideLlamaDecoderLayer", "GlideLlamaForCausalLM",
@@ -39,13 +40,6 @@ class GlideLlamaConfig(ModelConfig):
             self.large_head_dim = self.large_hidden_size // self.large_num_attention_heads
 
 
-def gather_paged_kv(cache: torch.Tensor, block_table: torch.Tensor, length: int) -> torch.Tensor:
-    """`cache` [blocks, block_size, Hkv, D] + one sequence's block table -> dense [length, Hkv, D]."""
-    bs = cache.shape[1]
-    nblk = (length + bs - 1) // bs
-    return cache[block_table[:nblk].long()].reshape(-1, cache.shape[2], cache.shape[3])[:length]
-
-
 class LlamaCrossAttention(nn.Module):
     """Queries from the drafter's hidden states, keys/values = the large model's cached K/V (no projection: the
     drafter learns to address the large model's key space directly)."""
@@ -67,8 +61,8 @@ class LlamaCrossAttention(nn.Module):
         outs = []
         for b in range(batch):
             L = int(glide.sequence_lengths[b])
-            k = gather_paged_kv(glide.large_k_cache, glide.block_tables[b], L).to(q.dtype)
-            v = gather_paged_kv(glide.large_v_cache, glide.block_tables[b], L).to(q.dtype)
+            k = gather_paged_kv(glide.large_k_cache, glide.block_tables[b], L, q.dtype)
+            v = gather_paged_kv(glide.large_v_cache, glide.block_tables[b], L, q.dtype)
             k = k.repeat_interleave(G, 1).transpose(0, 1)
             v = v.repeat_interleave(G, 1).transpose(0, 1)
             outs.append(F.scaled_dot_product_attention(q[b], k, v, scale=1.0 / math.sqrt(self.head_dim)))

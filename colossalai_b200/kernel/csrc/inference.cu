@@ -4,12 +4,14 @@
 // 16-byte vectors along head_dim; one (block, head) tile is a strided 2-D box, i.e. directly TMA-addressable).
 //
 //   cb_kv_cache_write        : scatter this step's K,V rows [tokens, kv_heads, D] into their paged slots (prefill: all
-//                              prompt tokens via cu_seqlens; decode: one token per sequence), optional fp8(e5m2) cast
+//                              prompt tokens via cu_seqlens; decode: one token per sequence); a 16-bit cache stores the
+//                              rows as they are, an fp8 cache (uint8 bytes) stores them rounded to e5m2
 //   cb_rope_kv_cache_write   : fused RoPE(q,k) in place + cache write of rotated K and of V (decode path)
 //   cb_paged_decode_attention: split-KV flash-decoding: grid (seq, group of <= 8 kv heads, split); one WARP serves a
 //                              kv head (its whole GQA group, so K/V are read once per group) and the warps of a CTA
 //                              stream adjacent head slices of the same token rows; fp32 online softmax; second pass
-//                              merges splits
+//                              merges splits; an e5m2 cache is decoded exactly to the query dtype after the load, so
+//                              the result is bitwise that of the 16-bit cache holding the decoded values
 //   cb_gather_cos_sin        : per-token cos/sin rows from the [max_pos, D/2] caches
 //   cb_convert_fp8           : fp16/bf16/fp32 <-> fp8 e5m2 storage
 //
@@ -39,6 +41,43 @@ CB_DEVICE float ex2_approx(float x) {
 }
 CB_DEVICE void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> CB_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// fp8 KV cache: a uint8 cache holds e5m2 bytes, written with round-to-nearest-even (as cb_convert_fp8 and
+// torch.float8_e5m2 do).  Every e5m2 value is exactly an fp16, bf16 and fp32 value, so decoding is exact.
+template <typename T> CB_DEVICE uint2 e5m2_pack8(const uint4 raw) {   // 8 values of T -> 8 e5m2 bytes
+  Vec16<T> x;
+  x.raw = raw;
+  uint32_t w[2];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(x.get(4 * j), x.get(4 * j + 1)), __NV_SATFINITE, __NV_E5M2);
+    const uint32_t hi =
+        __nv_cvt_float2_to_fp8x2(make_float2(x.get(4 * j + 2), x.get(4 * j + 3)), __NV_SATFINITE, __NV_E5M2);
+    w[j] = lo | (hi << 16);
+  }
+  return make_uint2(w[0], w[1]);
+}
+template <typename T> CB_DEVICE uint32_t e5m2x2_decode(uint32_t pair);   // 2 e5m2 bytes (low half) -> 2 values of T
+template <> CB_DEVICE uint32_t e5m2x2_decode<__half>(uint32_t pair) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)pair, __NV_E5M2);
+  return (uint32_t)h.x | ((uint32_t)h.y << 16);
+}
+template <> CB_DEVICE uint32_t e5m2x2_decode<__nv_bfloat16>(uint32_t pair) {
+  const float2 f = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)pair, __NV_E5M2)));
+  __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
+  return *reinterpret_cast<uint32_t*>(&b);
+}
+template <typename T> CB_DEVICE void e5m2_unpack16(const uint4 in, uint4 (&out)[2]) {   // 16 e5m2 bytes -> 16 of T
+  const uint32_t w[4] = {in.x, in.y, in.z, in.w};
+  uint32_t r[8];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    r[2 * j] = e5m2x2_decode<T>(w[j] & 0xffffu);
+    r[2 * j + 1] = e5m2x2_decode<T>(w[j] >> 16);
+  }
+  out[0] = make_uint4(r[0], r[1], r[2], r[3]);
+  out[1] = make_uint4(r[4], r[5], r[6], r[7]);
+}
 
 template <typename T, typename TC>
 __global__ void __launch_bounds__(256) kv_cache_write_kernel(const T* __restrict__ k, const T* __restrict__ v,
@@ -100,10 +139,11 @@ __global__ void __launch_bounds__(256) rope_kv_cache_write_kernel(T* __restrict_
 }
 
 // 16-byte vectorised variants (the hot ones): one thread moves one 16-byte vector, grid = all vectors of the step, so a
-// prefill of thousands of tokens is a single HBM-rate streaming kernel instead of one small CTA per token.
-template <typename T>
+// prefill of thousands of tokens is a single HBM-rate streaming kernel instead of one small CTA per token.  An e5m2
+// cache (TC = __nv_fp8_e5m2) takes the same 16 input bytes per thread and stores 8.
+template <typename T, typename TC>
 __global__ void __launch_bounds__(256) kv_cache_write_vec_kernel(const T* __restrict__ k, const T* __restrict__ v,
-                                                                 T* __restrict__ k_cache, T* __restrict__ v_cache,
+                                                                 TC* __restrict__ k_cache, TC* __restrict__ v_cache,
                                                                  const int* __restrict__ block_tables,
                                                                  const int* __restrict__ token_seq,
                                                                  const int* __restrict__ token_pos, int tokens,
@@ -118,10 +158,11 @@ __global__ void __launch_bounds__(256) kv_cache_write_vec_kernel(const T* __rest
     const int i = is_v ? r - vec_per_tok : r;
     const int seq = __ldg(token_seq + t), pos = __ldg(token_pos + t);
     const int blk = __ldg(block_tables + seq * max_blocks_per_seq + pos / block_size);
-    const int64_t dst = ((int64_t)blk * block_size + pos % block_size) * vec_per_tok + i;       // in 16-byte units
+    const int64_t dst = ((int64_t)blk * block_size + pos % block_size) * vec_per_tok + i;       // in 8-element units
     const uint4 val = is_v ? __ldg(reinterpret_cast<const uint4*>(v + (int64_t)t * v_stride) + i)
                            : __ldg(reinterpret_cast<const uint4*>(k + (int64_t)t * k_stride) + i);
-    reinterpret_cast<uint4*>(is_v ? v_cache : k_cache)[dst] = val;
+    if constexpr (sizeof(TC) == 1) reinterpret_cast<uint2*>(is_v ? v_cache : k_cache)[dst] = e5m2_pack8<T>(val);
+    else reinterpret_cast<uint4*>(is_v ? v_cache : k_cache)[dst] = val;
   }
 }
 
@@ -206,8 +247,11 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
     const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
     float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
     float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window) {
-  static_assert(sizeof(TC) == 2, "the paged cache is read as 16-byte vectors of 16-bit elements");
+  static_assert(sizeof(TC) == 2 || sizeof(TC) == 1, "16-bit or e5m2 cache");
   constexpr int EPL = 16;                       // elements of a row owned by a lane
+  // 16-byte vectors per lane and row: two of 16-bit elements, or one of e5m2 bytes (decoded to T after the load).  An
+  // e5m2 ring has twice the stages of half the size: the same shared memory and about the same bytes in flight.
+  constexpr int HV = sizeof(TC);
   constexpr int LPT = D / EPL;                  // lanes per token row: 4 / 8 / 16
   constexpr int TPW = 32 / LPT;                 // token rows per warp pass
   constexpr int GH = DEC_GH, U = DEC_U;
@@ -258,8 +302,8 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
   // lane reads back exactly the vectors it requested itself (slot = [stage][k|v][pass][half][lane]), so no barrier is
   // needed beyond cp.async.wait_group, and the 16-byte slots of a warp are consecutive (conflict-free LDS.128).
   extern __shared__ __align__(16) unsigned char dec_smem[];
-  constexpr int NST = DEC_STAGES;
-  constexpr int STAGE_VECS = 2 * U * 2 * 32;                      // uint4 slots per stage: (K|V) x pass x half x lane
+  constexpr int NST = DEC_STAGES * 2 / HV;
+  constexpr int STAGE_VECS = 2 * U * HV * 32;                     // uint4 slots per stage: (K|V) x pass x half x lane
   uint4* ring = reinterpret_cast<uint4*>(dec_smem) + (size_t)warp * NST * STAGE_VECS;
   auto issue_stage = [&](int base, int stage) {
     uint4* st = ring + stage * STAGE_VECS;
@@ -273,10 +317,22 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
       const int64_t row = (((int64_t)blk * block_size + slot) * Hkv + kvh) * D + sub * EPL;
       const uint32_t nbytes = ok ? 16u : 0u;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        cp_async_16(st + ((0 * U + u) * 2 + h) * 32 + lane, k_cache + row + h * 8, nbytes);
-        cp_async_16(st + ((1 * U + u) * 2 + h) * 32 + lane, v_cache + row + h * 8, nbytes);
+      for (int h = 0; h < HV; ++h) {
+        cp_async_16(st + ((0 * U + u) * HV + h) * 32 + lane, k_cache + row + h * 8, nbytes);
+        cp_async_16(st + ((1 * U + u) * HV + h) * 32 + lane, v_cache + row + h * 8, nbytes);
       }
+    }
+  };
+  // the lane's 16 elements of a K (kv = 0) or V (kv = 1) row of pass u, as two vectors of T
+  auto row_vecs = [&](const uint4* st, int kv, int u, Vec16<T>& a, Vec16<T>& b) {
+    if constexpr (HV == 1) {
+      uint4 x[2];
+      e5m2_unpack16<T>(st[(kv * U + u) * 32 + lane], x);
+      a.raw = x[0];
+      b.raw = x[1];
+    } else {
+      a.raw = st[((kv * U + u) * 2 + 0) * 32 + lane];
+      b.raw = st[((kv * U + u) * 2 + 1) * 32 + lane];
     }
   };
   auto consume = [&](int base, int stage) {
@@ -284,9 +340,8 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
     float sc[U][GH];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      Vec16<TC> k0, k1;
-      k0.raw = st[((0 * U + u) * 2 + 0) * 32 + lane];
-      k1.raw = st[((0 * U + u) * 2 + 1) * 32 + lane];
+      Vec16<T> k0, k1;
+      row_vecs(st, 0, u, k0, k1);
       const int t = base + u * TPW + grp;
 #pragma unroll
       for (int g = 0; g < GH; ++g) {
@@ -322,9 +377,8 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      Vec16<TC> v0, v1;
-      v0.raw = st[((1 * U + u) * 2 + 0) * 32 + lane];
-      v1.raw = st[((1 * U + u) * 2 + 1) * 32 + lane];
+      Vec16<T> v0, v1;
+      row_vecs(st, 1, u, v0, v1);
 #pragma unroll
       for (int g = 0; g < GH; ++g) {
 #pragma unroll
@@ -400,8 +454,16 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
 //     accumulator layout of S to the A-operand layout of P V (no shared-memory round trip); the output accumulator is
 //     rescaled only when a row max moved;
 //   * partial results use the same (o_part, ml_part) format, so the reduce kernel is shared.
+// An e5m2 cache (TC = __nv_fp8_e5m2) travels through the ring as bytes (half a 16-bit stage each, so 5 stages keep the
+// 16-bit ring's bytes in flight); the warp decodes the landed stage into one swizzled 16-bit K,V tile pair before the
+// ldmatrix reads, so the MMAs and everything after them are those of the 16-bit kernel.
 constexpr int DEC_MMA_TOKENS = 16;
 constexpr int DEC_MMA_STAGES = 3;
+
+template <typename TC> constexpr int dec_mma_stages() { return sizeof(TC) == 1 ? 5 : DEC_MMA_STAGES; }
+template <typename TC, int D> constexpr int dec_mma_smem_per_warp() {
+  return dec_mma_stages<TC>() * 2 * DEC_MMA_TOKENS * D * (int)sizeof(TC) + (sizeof(TC) == 1 ? 2 * DEC_MMA_TOKENS * D * 2 : 0);
+}
 
 CB_DEVICE void ldmatrix_x4(uint32_t (&r)[4], const void* smem_row) {
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_row);
@@ -434,18 +496,21 @@ template <> CB_DEVICE uint32_t pack2<__half>(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <typename T, int D>
+template <typename T, typename TC, int D>
 __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
-    const T* __restrict__ q, const T* __restrict__ k_cache, const T* __restrict__ v_cache,
+    const T* __restrict__ q, const TC* __restrict__ k_cache, const TC* __restrict__ v_cache,
     const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
     float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
     float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window) {
-  constexpr int NT = DEC_MMA_TOKENS, NST = DEC_MMA_STAGES;
+  static_assert(sizeof(TC) == 2 || sizeof(TC) == 1, "16-bit or e5m2 cache");
+  constexpr bool F8 = sizeof(TC) == 1;
+  constexpr int NT = DEC_MMA_TOKENS, NST = dec_mma_stages<TC>();
   constexpr int KS = D / 16;                    // k-steps of Q K^T
   constexpr int NO = D / 8;                     // 8-wide column tiles of the output
-  constexpr int CPR = D / 8;                    // 16-byte chunks per token row
-  constexpr int ROW_BYTES = D * 2;
-  constexpr int TILE_BYTES = NT * ROW_BYTES;    // one operand (K or V) of one stage
+  constexpr int CPR = D * (int)sizeof(TC) / 16; // 16-byte chunks per cached token row
+  constexpr int ROW_BYTES = D * 2;              // a token row of a 16-bit tile
+  constexpr int TILE_BYTES = NT * ROW_BYTES;    // one 16-bit operand (K or V) tile
+  constexpr int STAGE_BYTES = 2 * NT * D * (int)sizeof(TC);   // K and V of one stage as cached
   constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
   const int seq = blockIdx.x, split = blockIdx.z;
   const int G = Hq / Hkv;
@@ -478,12 +543,13 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
   float m_run = -INFINITY, l_run = 0.f;         // per head row, replicated over the quad (l: this lane's share)
 
   extern __shared__ __align__(128) unsigned char dec_smem[];
-  unsigned char* ring = dec_smem + (size_t)warp * NST * 2 * TILE_BYTES;
+  unsigned char* ring = dec_smem + (F8 ? (size_t)warp * dec_mma_smem_per_warp<TC, D>() : (size_t)warp * NST * 2 * TILE_BYTES);
+  unsigned char* decoded = ring + NST * STAGE_BYTES;         // e5m2: the stage being consumed, as a 16-bit K,V tile
   const int* bt = block_tables + seq * max_blocks_per_seq;
   const int bs_shift = (block_size & (block_size - 1)) == 0 ? 31 - __clz(block_size) : -1;
   auto issue_stage = [&](int base, int stage) {
-    unsigned char* kt = ring + (size_t)stage * 2 * TILE_BYTES;
-    unsigned char* vt = kt + TILE_BYTES;
+    unsigned char* kt = ring + (size_t)stage * STAGE_BYTES;
+    unsigned char* vt = kt + STAGE_BYTES / 2;
 #pragma unroll
     for (int i = 0; i < NT * CPR / 32; ++i) {
       const int cid = lane + 32 * i;
@@ -493,15 +559,31 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
       const int tt = ok ? t : t0;
       const int blk = bt[bs_shift >= 0 ? (tt >> bs_shift) : (tt / block_size)];
       const int slot = bs_shift >= 0 ? (tt & (block_size - 1)) : (tt % block_size);
-      const int64_t src = (((int64_t)blk * block_size + slot) * Hkv + kvh) * D + c * 8;
-      const int dst = tr * ROW_BYTES + ((c ^ (tr & 7)) << 4);
+      const int64_t src = (((int64_t)blk * block_size + slot) * Hkv + kvh) * D + c * (16 / (int)sizeof(TC));
+      const int dst = F8 ? tr * D + (c << 4) : tr * ROW_BYTES + ((c ^ (tr & 7)) << 4);   // e5m2 bytes: unswizzled
       const uint32_t nbytes = ok ? 16u : 0u;
       cp_async_16(kt + dst, k_cache + src, nbytes);
       cp_async_16(vt + dst, v_cache + src, nbytes);
     }
   };
+  // e5m2 stage -> `decoded`: each lane decodes the chunks it loaded into the 16-bit tiles' swizzled layout
+  auto decode_stage = [&](const unsigned char* kt8) {
+#pragma unroll
+    for (int i = 0; i < NT * CPR / 32; ++i) {
+      const int cid = lane + 32 * i;
+      const int tr = cid / CPR, c = cid - tr * CPR;
+#pragma unroll
+      for (int kv = 0; kv < 2; ++kv) {
+        uint4 x[2];
+        e5m2_unpack16<T>(*reinterpret_cast<const uint4*>(kt8 + kv * (STAGE_BYTES / 2) + tr * D + (c << 4)), x);
+        unsigned char* row16 = decoded + kv * TILE_BYTES + tr * ROW_BYTES;
+        *reinterpret_cast<uint4*>(row16 + (((2 * c) ^ (tr & 7)) << 4)) = x[0];
+        *reinterpret_cast<uint4*>(row16 + (((2 * c + 1) ^ (tr & 7)) << 4)) = x[1];
+      }
+    }
+  };
   auto consume = [&](int base, int stage) {
-    const unsigned char* kt = ring + (size_t)stage * 2 * TILE_BYTES;
+    const unsigned char* kt = F8 ? decoded : ring + (size_t)stage * STAGE_BYTES;
     const unsigned char* vt = kt + TILE_BYTES;
     // ---- S = Q K^T for 16 tokens (two 8-token column tiles)
     float sacc[2][4];
@@ -580,6 +662,10 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
       cp_async_commit();
       cp_async_wait<NST - 1>();
       __syncwarp();                                          // the tile was written by all lanes of the warp
+      if constexpr (F8) {
+        decode_stage(ring + (size_t)(it % NST) * STAGE_BYTES);
+        __syncwarp();                                        // the decoded tile was written by all lanes
+      }
       consume(base, it % NST);
       __syncwarp();                                          // all lanes done reading before the stage is refilled
     }
@@ -641,28 +727,40 @@ __global__ void convert_kernel(const TI* __restrict__ in, TO* __restrict__ out, 
 
 extern "C" {
 
-// k, v: [tokens, kv_heads, D] (row strides in elements).  cache dtype == input dtype (fp8 path: cb_convert_fp8 first).
+// k, v: [tokens, kv_heads, D] (row strides in elements) of `dtype`; the caches hold `cache_dtype`: the same dtype, or
+// CB_F8E5M2 (e5m2 bytes, rounded to nearest even).
 int cb_kv_cache_write(const void* k, const void* v, void* k_cache, void* v_cache, const int* block_tables,
                       const int* token_seq, const int* token_pos, int tokens, int kv_heads, int D, int block_size,
-                      int max_blocks_per_seq, int64_t k_stride, int64_t v_stride, int dtype, cudaStream_t s) {
+                      int max_blocks_per_seq, int64_t k_stride, int64_t v_stride, int dtype, int cache_dtype,
+                      cudaStream_t s) {
   if (tokens == 0) return 0;
+  if (cache_dtype != dtype && cache_dtype != CB_F8E5M2) return (int)cudaErrorInvalidValue;
+  const bool f8 = cache_dtype == CB_F8E5M2;
   const int n = kv_heads * D;
   if (n % 8 == 0 && k_stride % 8 == 0 && v_stride % 8 == 0 && ((uintptr_t)k % 16) == 0 && ((uintptr_t)v % 16) == 0 &&
       ((uintptr_t)k_cache % 16) == 0 && ((uintptr_t)v_cache % 16) == 0) {
     const int64_t total = (int64_t)tokens * 2 * (n / 8);
     const int grid = (int)((total + 255) / 256 < 16 * cb_num_sms() ? (total + 255) / 256 : 16 * cb_num_sms());
+#define LAUNCH_KV_WRITE_VEC(TC)                                                                                       \
+  kv_cache_write_vec_kernel<T, TC><<<grid, 256, 0, s>>>((const T*)k, (const T*)v, (TC*)k_cache, (TC*)v_cache,           \
+                                                        block_tables, token_seq, token_pos, tokens, n / 8, block_size, \
+                                                        max_blocks_per_seq, k_stride, v_stride)
     CB_DISPATCH_HALF(dtype, T, {
-      kv_cache_write_vec_kernel<T><<<grid, 256, 0, s>>>((const T*)k, (const T*)v, (T*)k_cache, (T*)v_cache, block_tables,
-                                                       token_seq, token_pos, tokens, n / 8, block_size,
-                                                       max_blocks_per_seq, k_stride, v_stride);
+      if (f8) LAUNCH_KV_WRITE_VEC(__nv_fp8_e5m2);
+      else LAUNCH_KV_WRITE_VEC(T);
     });
+#undef LAUNCH_KV_WRITE_VEC
     return CB_LAUNCH_CHECK();
   }
+#define LAUNCH_KV_WRITE(TC)                                                                                           \
+  kv_cache_write_kernel<T, TC><<<tokens, 256, 0, s>>>((const T*)k, (const T*)v, (TC*)k_cache, (TC*)v_cache,             \
+                                                      block_tables, token_seq, token_pos, tokens, kv_heads, D,         \
+                                                      block_size, max_blocks_per_seq, k_stride, v_stride)
   CB_DISPATCH_HALF(dtype, T, {
-    kv_cache_write_kernel<T, T><<<tokens, 256, 0, s>>>((const T*)k, (const T*)v, (T*)k_cache, (T*)v_cache, block_tables,
-                                                      token_seq, token_pos, tokens, kv_heads, D, block_size,
-                                                      max_blocks_per_seq, k_stride, v_stride);
+    if (f8) LAUNCH_KV_WRITE(__nv_fp8_e5m2);
+    else LAUNCH_KV_WRITE(T);
   });
+#undef LAUNCH_KV_WRITE
   return CB_LAUNCH_CHECK();
 }
 
@@ -709,14 +807,16 @@ int cb_decode_num_splits(int num_seqs, int kv_heads, int max_len, int* part_len_
   return splits;
 }
 
-// q: [num_seqs, Hq, D]; out same; caches [nb, bs, Hkv, D]; o_part fp32 [num_seqs, Hq, splits, D]; ml_part [.., 2]
+// q: [num_seqs, Hq, D] of `dtype`; out same; caches [nb, bs, Hkv, D] of `cache_dtype` (`dtype` or CB_F8E5M2);
+// o_part fp32 [num_seqs, Hq, splits, D]; ml_part [.., 2]
 int cb_paged_decode_attention(const void* q, const void* k_cache, const void* v_cache, const int* block_tables,
                               const int* seq_lens, void* out, float* o_part, float* ml_part, int num_seqs, int Hq,
                               int Hkv, int D, int block_size, int max_blocks_per_seq, int splits, int part_len,
                               float scale, const float* alibi_slopes, int64_t q_stride, int64_t out_stride, int dtype,
-                              int window, cudaStream_t s) {
+                              int cache_dtype, int window, cudaStream_t s) {
   if (num_seqs == 0) return 0;
   if (Hq % Hkv != 0 || Hq / Hkv > MAX_GROUP) return (int)cudaErrorInvalidValue;
+  if (cache_dtype != dtype && cache_dtype != CB_F8E5M2) return (int)cudaErrorInvalidValue;
   const int G = Hq / Hkv;
   const int units = Hkv * ((G + DEC_GH - 1) / DEC_GH);             // (kv head, query-head set) pairs = warps needed
   const int warps = units < DEC_THREADS / 32 ? units : DEC_THREADS / 32;
@@ -729,40 +829,44 @@ int cb_paged_decode_attention(const void* q, const void* k_cache, const void* v_
   const bool use_mma = !(impl_env != nullptr && impl_env[0] == 's') && G <= 8 && (D == 128 || D == 64);
   const int mma_warps = Hkv < DEC_THREADS / 32 ? Hkv : DEC_THREADS / 32;
   dim3 mma_grid(num_seqs, (Hkv + mma_warps - 1) / mma_warps, splits);
-#define LAUNCH_DEC_MMA(T, DD)                                                                                       \
+#define LAUNCH_DEC_MMA(T, TC, DD)                                                                                   \
   {                                                                                                                  \
-    constexpr int per_warp = DEC_MMA_STAGES * 2 * DEC_MMA_TOKENS * DD * 2;                                           \
+    constexpr int per_warp = dec_mma_smem_per_warp<TC, DD>();                                                        \
     static bool attr_done = false;                                                                                   \
     if (!attr_done) {                                                                                                \
-      cudaFuncSetAttribute(paged_decode_mma_kernel<T, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,              \
+      cudaFuncSetAttribute(paged_decode_mma_kernel<T, TC, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
                            (DEC_THREADS / 32) * per_warp);                                                           \
       attr_done = true;                                                                                              \
     }                                                                                                                \
-    paged_decode_mma_kernel<T, DD><<<mma_grid, mma_warps * 32, mma_warps * per_warp, s>>>(                           \
-        (const T*)q, (const T*)k_cache, (const T*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv,        \
+    paged_decode_mma_kernel<T, TC, DD><<<mma_grid, mma_warps * 32, mma_warps * per_warp, s>>>(                       \
+        (const T*)q, (const TC*)k_cache, (const TC*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv,      \
         block_size, max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window);                   \
     decode_reduce_kernel<T, DD><<<dim3(num_seqs, Hq), 128, 0, s>>>(o_part, ml_part, (T*)out, Hq, splits, out_stride); \
   }
-#define LAUNCH_DEC(T, DD)                                                                                           \
+#define LAUNCH_DEC(T, TC, DD)                                                                                       \
   {                                                                                                                  \
     static bool attr_done = false;                                                                                   \
     if (!attr_done) {                                                                                                \
-      cudaFuncSetAttribute(paged_decode_kernel<T, T, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, dec_smem_max);\
+      cudaFuncSetAttribute(paged_decode_kernel<T, TC, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, dec_smem_max);\
       attr_done = true;                                                                                              \
     }                                                                                                                \
   }                                                                                                                  \
-  paged_decode_kernel<T, T, DD><<<grid, warps * 32, dec_smem, s>>>((const T*)q, (const T*)k_cache, (const T*)v_cache, \
-      block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size, max_blocks_per_seq, splits, part_len, scale,     \
-      alibi_slopes, q_stride, window);                                                                               \
+  paged_decode_kernel<T, TC, DD><<<grid, warps * 32, dec_smem, s>>>((const T*)q, (const TC*)k_cache,                 \
+      (const TC*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size, max_blocks_per_seq, splits,  \
+      part_len, scale, alibi_slopes, q_stride, window);                                                              \
   decode_reduce_kernel<T, DD><<<dim3(num_seqs, Hq), 128, 0, s>>>(o_part, ml_part, (T*)out, Hq, splits, out_stride)
+#define DISPATCH_DEC_D(T, TC)                                                                                       \
+  if (use_mma && D == 128) { LAUNCH_DEC_MMA(T, TC, 128); }                                                           \
+  else if (use_mma && D == 64) { LAUNCH_DEC_MMA(T, TC, 64); }                                                        \
+  else if (D == 128) { LAUNCH_DEC(T, TC, 128); }                                                                     \
+  else if (D == 64) { LAUNCH_DEC(T, TC, 64); }                                                                       \
+  else if (D == 256) { LAUNCH_DEC(T, TC, 256); }                                                                     \
+  else return (int)cudaErrorInvalidValue;
   CB_DISPATCH_HALF(dtype, T, {
-    if (use_mma && D == 128) { LAUNCH_DEC_MMA(T, 128); }
-    else if (use_mma && D == 64) { LAUNCH_DEC_MMA(T, 64); }
-    else if (D == 128) { LAUNCH_DEC(T, 128); }
-    else if (D == 64) { LAUNCH_DEC(T, 64); }
-    else if (D == 256) { LAUNCH_DEC(T, 256); }
-    else return (int)cudaErrorInvalidValue;
+    if (cache_dtype == CB_F8E5M2) { DISPATCH_DEC_D(T, __nv_fp8_e5m2) }
+    else { DISPATCH_DEC_D(T, T) }
   });
+#undef DISPATCH_DEC_D
 #undef LAUNCH_DEC
 #undef LAUNCH_DEC_MMA
   return CB_LAUNCH_CHECK();

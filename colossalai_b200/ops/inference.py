@@ -1,5 +1,10 @@
 """Python face of the paged-KV inference kernels (kernel/csrc/inference.cu) with PyTorch reference paths.
-Parity: reference `inference_ops_cuda` bindings used by `inference/modeling/backends/*.py`."""
+Parity: reference `inference_ops_cuda` bindings used by `inference/modeling/backends/*.py`.
+
+KV-cache format: a floating-point cache holds the K/V values as they are; a `torch.uint8` cache is the fp8 cache and
+holds fp8 e5m2 bytes (round to nearest even on write; every e5m2 value decodes exactly to fp16, bf16 and fp32).  This
+module is the only one that interprets those bytes: the runtime, engine and drafters write and read the cache through
+`kv_cache_write`, `paged_decode_attention` and `gather_paged_kv`."""
 from __future__ import annotations
 
 import ctypes
@@ -22,24 +27,57 @@ def _get_lib():
     return _lib
 
 
+FP8_CACHE_DTYPE = torch.uint8          # storage dtype of an fp8 (e5m2) KV cache
+
+
+def _cache_code(cache: torch.Tensor) -> int:
+    return code(torch.float8_e5m2 if cache.dtype == FP8_CACHE_DTYPE else cache.dtype)
+
+
+def _encode(x: torch.Tensor, cache_dtype: torch.dtype) -> torch.Tensor:
+    """Values -> what a cache of `cache_dtype` stores."""
+    if cache_dtype == FP8_CACHE_DTYPE:
+        return x.to(torch.float8_e5m2).view(FP8_CACHE_DTYPE)
+    return x.to(cache_dtype)
+
+
+def _decode(stored: torch.Tensor, dtype: Optional[torch.dtype]) -> torch.Tensor:
+    """What a cache stores -> values of `dtype` (None: the stored values' own dtype, torch.float8_e5m2 for fp8)."""
+    if stored.dtype == FP8_CACHE_DTYPE:
+        stored = stored.view(torch.float8_e5m2)
+    return stored if dtype is None else stored.to(dtype)
+
+
 def kv_cache_write(k: torch.Tensor, v: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
                    block_tables: torch.Tensor, token_seq: torch.Tensor, token_pos: torch.Tensor) -> None:
-    """k, v: [tokens, Hkv, D] -> caches [nb, bs, Hkv, D] at (block_tables[seq][pos // bs], pos % bs)."""
+    """k, v: [tokens, Hkv, D] -> caches [nb, bs, Hkv, D] at (block_tables[seq][pos // bs], pos % bs).  A uint8 cache
+    stores the values rounded to fp8 e5m2."""
     tokens, Hkv, D = k.shape
     bs = k_cache.shape[1]
-    if use_native(k) and k.dtype in (torch.float16, torch.bfloat16) and k_cache.dtype == k.dtype:
+    if (use_native(k) and k.dtype in (torch.float16, torch.bfloat16)
+            and k_cache.dtype in (k.dtype, FP8_CACHE_DTYPE)):
         lib = _get_lib()
         loader.check(lib.cb_kv_cache_write(loader.ptr(k), loader.ptr(v), loader.ptr(k_cache), loader.ptr(v_cache),
                                            loader.ptr(block_tables), loader.ptr(token_seq), loader.ptr(token_pos),
                                            tokens, Hkv, D, bs, block_tables.shape[1], ctypes.c_int64(k.stride(0)),
-                                           ctypes.c_int64(v.stride(0)), code(k.dtype), loader.stream_ptr()),
+                                           ctypes.c_int64(v.stride(0)), code(k.dtype), _cache_code(k_cache),
+                                           loader.stream_ptr()),
                      "kv_cache_write")
         loader.launch_counter.add("kv_cache_write")
         return
     blk = block_tables[token_seq.long(), (token_pos // bs).long()].long()
     slot = (token_pos % bs).long()
-    k_cache[blk, slot] = k.to(k_cache.dtype)
-    v_cache[blk, slot] = v.to(v_cache.dtype)
+    k_cache[blk, slot] = _encode(k, k_cache.dtype)
+    v_cache[blk, slot] = _encode(v, v_cache.dtype)
+
+
+def gather_paged_kv(cache: torch.Tensor, block_table: torch.Tensor, length: int,
+                    dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """One sequence's cached K or V: `cache` [blocks, block_size, Hkv, D] + its block table -> dense [length, Hkv, D]
+    values, as `dtype` (None: the cache's value dtype; torch.float8_e5m2 for an fp8 cache)."""
+    bs = cache.shape[1]
+    nblk = (length + bs - 1) // bs
+    return _decode(cache[block_table[:nblk].long()].reshape(-1, cache.shape[2], cache.shape[3])[:length], dtype)
 
 
 def _decode_workspace(q: torch.Tensor, n: int, heads: int, splits: int, head_dim: int):
@@ -56,11 +94,12 @@ def paged_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torc
                            seq_lens: torch.Tensor, scale: Optional[float] = None,
                            alibi_slopes: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
     """q: [num_seqs, Hq, D] (one new token per sequence) -> [num_seqs, Hq, D].  `window`: sliding-window attention
-    (only the last `window` cached tokens are visible), handled inside the split-KV kernel (`window_start`)."""
+    (only the last `window` cached tokens are visible), handled inside the split-KV kernel (`window_start`).  An fp8
+    (uint8) cache is decoded exactly to the query dtype inside the kernel."""
     n, Hq, D = q.shape
     nb, bs, Hkv, _ = k_cache.shape
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
-    if (use_native(q) and q.dtype in (torch.float16, torch.bfloat16) and k_cache.dtype == q.dtype
+    if (use_native(q) and q.dtype in (torch.float16, torch.bfloat16) and k_cache.dtype in (q.dtype, FP8_CACHE_DTYPE)
             and D in (64, 128, 256) and Hq // Hkv <= 8):
         lib = _get_lib()
         max_len = block_tables.shape[1] * bs
@@ -78,7 +117,7 @@ def paged_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torc
             loader.ptr(qc), loader.ptr(k_cache), loader.ptr(v_cache), loader.ptr(block_tables), loader.ptr(seq_lens),
             loader.ptr(out), loader.ptr(o_part), loader.ptr(ml_part), n, Hq, Hkv, D, bs, block_tables.shape[1], splits,
             part.value, ctypes.c_float(scale), loader.ptr(alibi_slopes), ctypes.c_int64(qc.stride(0)),
-            ctypes.c_int64(out.stride(0)), code(q.dtype), int(window or 0), loader.stream_ptr()),
+            ctypes.c_int64(out.stride(0)), code(q.dtype), _cache_code(k_cache), int(window or 0), loader.stream_ptr()),
             "paged_decode_attention")
         loader.launch_counter.add("paged_decode_attention", 2)
         return out
@@ -94,10 +133,8 @@ def paged_decode_attention_ref(q, k_cache, v_cache, block_tables, seq_lens, scal
     out = torch.empty_like(q)
     for i in range(n):
         L = int(seq_lens[i])
-        nblk = (L + bs - 1) // bs
-        blks = block_tables[i, :nblk].long()
-        k = k_cache[blks].reshape(-1, Hkv, D)[:L].float()
-        v = v_cache[blks].reshape(-1, Hkv, D)[:L].float()
+        k = gather_paged_kv(k_cache, block_tables[i], L, torch.float32)
+        v = gather_paged_kv(v_cache, block_tables[i], L, torch.float32)
         if window is not None and L > window:
             k, v, L = k[L - window:], v[L - window:], window
         k = k.repeat_interleave(G, dim=1)
@@ -120,11 +157,11 @@ def convert_fp8(x: torch.Tensor, to_fp8: bool, out_dtype: torch.dtype = torch.bf
                          "convert_fp8")
             loader.launch_counter.add("convert_fp8")
             return out
-        return x.to(torch.float8_e5m2).view(torch.uint8)
+        return _encode(x, FP8_CACHE_DTYPE)
     if use_native(x):
         out = torch.empty(x.shape, dtype=out_dtype, device=x.device)
         loader.check(_get_lib().cb_convert_fp8(loader.ptr(x.contiguous()), loader.ptr(out), ctypes.c_int64(x.numel()),
                                                code(out_dtype), 1, loader.stream_ptr()), "convert_fp8")
         loader.launch_counter.add("convert_fp8")
         return out
-    return x.view(torch.float8_e5m2).to(out_dtype)
+    return _decode(x, out_dtype)
