@@ -130,9 +130,10 @@ class LLMEngine(BaseEngine):
         assert isinstance(self.inference_config, InferenceConfig), "Invalid type of inference config provided."
         assert isinstance(self.model, nn.Module), f"the model type must be nn.Module, but got {type(self.model)}"
 
-    def _init_decode_workspace(self, k_caches) -> None:
+    def _init_decode_workspace(self, k_caches, q_per_seq: int = 1) -> None:
         """Size the persistent split-KV buffers of the paged decode kernel for the largest batch (reference
-        `flash_decoding_utils.FDIntermTensors.initialize` called from the request handler)."""
+        `flash_decoding_utils.FDIntermTensors.initialize` called from the request handler); `q_per_seq` query tokens
+        per sequence (speculative verification) need that many rows of partials per sequence."""
         if not torch.cuda.is_available() or not k_caches or k_caches[0].device.type != "cuda":
             return
         import ctypes
@@ -148,7 +149,7 @@ class LLMEngine(BaseEngine):
         try:
             lib = infer_ops._get_lib()
             part = ctypes.c_int(0)
-            worst = max(n * lib.cb_decode_num_splits(n, hkv, max_len, ctypes.byref(part))
+            worst = max(n * q_per_seq * lib.cb_decode_num_splits(n, hkv, max_len, ctypes.byref(part))
                         for n in range(1, cfg.max_batch_size + 1))
             FDIntermTensors().ensure(worst, hq, d, device=k_caches[0].device)
         except Exception as e:                # extension not built / odd config: the op allocates per call instead
@@ -202,6 +203,7 @@ class LLMEngine(BaseEngine):
             self.drafter_model = drafter_model.to(self.dtype).to(self.device).eval()
             self.drafter = Drafter(self.drafter_model, self.tokenizer, device=self.device, dtype=self.dtype)
         self.use_glide = use_glide_drafter
+        self._init_decode_workspace(self.kv_runtime.k_caches, q_per_seq=self.n_spec_tokens + 1)   # verify pass
         self.request_handler.set_spec_dec_mode(self.n_spec_tokens)
         self.use_spec_dec = True
 
@@ -245,7 +247,7 @@ class LLMEngine(BaseEngine):
         batch._sequence_lengths[: len(seqs)] += n
         # 2) verify: feed last accepted token + n drafted tokens (n+1 queries per sequence)
         batch.set_use_spec_dec(n)
-        input_ids = batch.get_1D_inputs()
+        input_ids = batch.get_1D_inputs().to(self.device)
         lens = batch.get_sequence_lengths()
         positions = self.kv_runtime.set_step(batch.get_block_table_tensor(), lens, False, self.device, q_per_seq=n + 1)
         from ...models.transformer import SeqMeta

@@ -97,18 +97,8 @@ class PagedKVRuntime:
                 bias = bias.masked_fill(~keep[None], float("-inf")).to(q.dtype)[None]
                 outs.append(attention_ref(q[a:b], k[a:b], v[a:b], batch=1, causal=False, scale=scale, attn_mask=bias))
             return torch.cat(outs, 0)
-        n = self.q_per_seq
-        if n == 1:
-            return iops.paged_decode_attention(q, kc, vc, self.block_tables, self.seq_lens, scale,
-                                               alibi_slopes=alibi_slopes, window=window)
-        bsz = self.seq_lens.numel()
-        outs = []
-        for j in range(n):
-            qj = q.view(bsz, n, *q.shape[1:])[:, j]
-            outs.append(iops.paged_decode_attention(qj.contiguous(), kc, vc, self.block_tables,
-                                                    self.seq_lens - (n - 1 - j), scale, alibi_slopes=alibi_slopes,
-                                                    window=window))
-        return torch.stack(outs, 1).reshape(q.shape)
+        return iops.paged_decode_attention(q, kc, vc, self.block_tables, self.seq_lens, scale,
+                                           alibi_slopes=alibi_slopes, window=window, q_len=self.q_per_seq)
 
     def _attend_full(self, q, k, v, kc, vc, scale, alibi_slopes) -> torch.Tensor:
         if alibi_slopes is not None:
@@ -123,20 +113,11 @@ class PagedKVRuntime:
                 md = AttentionMetaData(q, k, v, kc, vc, self.block_tables, self.block_size, cu_seqlens=self.cu_seqlens,
                                        sm_scale=scale, alibi_slopes=alibi_slopes)
                 return ReferenceAttentionBackend().prefill(md)
-            assert self.q_per_seq == 1, "speculative verification is not implemented for ALiBi models"
             return iops.paged_decode_attention(q, kc, vc, self.block_tables, self.seq_lens, scale,
-                                               alibi_slopes=alibi_slopes)
+                                               alibi_slopes=alibi_slopes, q_len=self.q_per_seq)
         if self.is_prompt:
             return ops.attention(q, k, v, causal=True, scale=scale, cu_seqlens_q=self.cu_seqlens,
                                  cu_seqlens_k=self.cu_seqlens, max_seqlen=self.max_seqlen)
-        if self.q_per_seq == 1:
-            return iops.paged_decode_attention(q, kc, vc, self.block_tables, self.seq_lens, scale)
-        # speculative verification: n query tokens per sequence, each sees the cache up to its own position
-        n = self.q_per_seq
-        bsz = self.seq_lens.numel()
-        outs = []
-        for j in range(n):
-            qj = q.view(bsz, n, *q.shape[1:])[:, j]
-            outs.append(iops.paged_decode_attention(qj.contiguous(), kc, vc, self.block_tables,
-                                                    self.seq_lens - (n - 1 - j), scale))
-        return torch.stack(outs, 1).reshape(q.shape)
+        # decode (q_per_seq = 1) or speculative verification (q_per_seq tokens per sequence, each sees the cache up to
+        # its own position): one pass over the cache either way
+        return iops.paged_decode_attention(q, kc, vc, self.block_tables, self.seq_lens, scale, q_len=self.q_per_seq)

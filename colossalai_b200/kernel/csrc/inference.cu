@@ -12,6 +12,10 @@
 //                              stream adjacent head slices of the same token rows; fp32 online softmax; second pass
 //                              merges splits; an e5m2 cache is decoded exactly to the query dtype after the load, so
 //                              the result is bitwise that of the 16-bit cache holding the decoded values
+//   cb_paged_verify_attention: the same split-KV pass for q_len <= 16 query tokens per sequence (speculative
+//                              verification): the MMA rows are (query token, q head) pairs, so up to 16 / G tokens cost
+//                              one decode pass over K/V; each token sees the cache up to its own position, and without a
+//                              window each output row is bitwise the decode kernel's result for that token alone
 //   cb_gather_cos_sin        : per-token cos/sin rows from the [max_pos, D/2] caches
 //   cb_convert_fp8           : fp16/bf16/fp32 <-> fp8 e5m2 storage
 //
@@ -496,12 +500,20 @@ template <> CB_DEVICE uint32_t pack2<__half>(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <typename T, typename TC, int D>
-__global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
+// Multi-query form (MQ, speculative verification): q_len query tokens per sequence, q / out rows seq * q_len + j.  The
+// MMA rows are the flattened (query token j, q head g) pairs r = j * G + g, all 16 of them used; a warp is one (kv head,
+// 16-row slice) unit, and when q_len * G > 16 the sibling warps of a kv head stream (and, for e5m2, decode) the same K/V
+// tiles, meant to hit L1 / L2 on the second read.  Query j sees the len_j = len - (q_len - 1 - j) first positions (the last `window` of them); each
+// row masks its own range, the tiles keep their bases at split * part_len and run to the warp's longest row, and a
+// masked position adds p = 0 - so without a window each row is bitwise the decode kernel's result for that row alone.
+// A window starts the tile grid at the warp's first row's window start, so windowed rows match only to rounding.
+// The decode kernel is the MQ = false instantiation with q_len = 1 (the upper 8 MMA rows stay zero padding).
+template <typename T, typename TC, int D, bool MQ>
+CB_DEVICE void paged_mma_attend(
     const T* __restrict__ q, const TC* __restrict__ k_cache, const TC* __restrict__ v_cache,
     const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
     float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
-    float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window) {
+    float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window, int q_len) {
   static_assert(sizeof(TC) == 2 || sizeof(TC) == 1, "16-bit or e5m2 cache");
   constexpr bool F8 = sizeof(TC) == 1;
   constexpr int NT = DEC_MMA_TOKENS, NST = dec_mma_stages<TC>();
@@ -515,20 +527,60 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
   const int seq = blockIdx.x, split = blockIdx.z;
   const int G = Hq / Hkv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kvh = blockIdx.y * (blockDim.x >> 5) + warp;
+  const int nrows = q_len * G;                  // MMA rows of a kv head: (query token, q head) pairs
+  const int nslices = MQ ? (nrows + 15) >> 4 : 1;
+  const int unit = blockIdx.y * (blockDim.x >> 5) + warp;
+  const int kvh = unit / nslices, r0 = (unit - kvh * nslices) * 16;   // kv head, first MMA row of the warp's slice
   if (kvh >= Hkv) return;                       // (no block-wide barrier in this kernel)
   const int len = seq_lens[seq];
-  const int window_start = window > 0 ? max(0, len - window) : 0;
-  const int t0 = max(split * part_len, window_start), t1 = min(len, split * part_len + part_len);
+  // positions [lo, hi) of this partition that query token j sees
+  auto visible = [&](int j, int& lo, int& hi) {
+    const int len_j = len - (q_len - 1 - j);
+    const int window_start = window > 0 ? max(0, len_j - window) : 0;
+    lo = max(split * part_len, window_start);
+    hi = min(len_j, split * part_len + part_len);
+  };
+  int t0, t1, unused;                           // the warp's tile range: first row's start to last row's end
+  visible(MQ ? r0 / G : 0, t0, unused);
+  visible(MQ ? (min(nrows, r0 + 16) - 1) / G : 0, unused, t1);
   const int row = lane >> 2, quad = lane & 3;   // accumulator layout: head row, column pair inside an 8-wide tile
   const bool row_ok = row < G;                  // rows G..15 of the MMA are padding
   const float scale2 = scale * LOG2E;           // scores in the exp2 domain
   const float slope2 = (alibi_slopes != nullptr && row_ok) ? alibi_slopes[kvh * G + row] * LOG2E : 0.f;
   const bool has_alibi = alibi_slopes != nullptr;
+  // MQ: this lane's two MMA rows, r0 + row (h = 0, accumulator regs 0 / 1) and r0 + row + 8 (h = 1, regs 2 / 3)
+  bool rok[2];
+  int rq[2], rhead[2], rlen[2], rlo[2], rhi[2];
+  float rslope[2];
+  if constexpr (MQ) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + row + 8 * h;
+      rok[h] = r < nrows;
+      rq[h] = rok[h] ? r / G : 0;
+      rhead[h] = kvh * G + (rok[h] ? r - rq[h] * G : 0);
+      rlen[h] = len - (q_len - 1 - rq[h]);
+      visible(rq[h], rlo[h], rhi[h]);
+      if (!rok[h]) rlo[h] = rhi[h] = 0;         // padding row: every position masked
+      rslope[h] = (alibi_slopes != nullptr && rok[h]) ? alibi_slopes[rhead[h]] * LOG2E : 0.f;
+    }
+  }
 
-  // ---- Q fragments: A operand [16 heads x 16 d] per k-step; a1 / a3 are head rows 8..15 = zero (G <= 8)
+  // ---- Q fragments: A operand [16 rows x 16 d] per k-step; decode: a1 / a3 are head rows 8..15 = zero (G <= 8)
   uint32_t qa[KS][4];
-  {
+  if constexpr (MQ) {
+    const T* qr0 = q + (int64_t)(seq * q_len + rq[0]) * q_stride + (int64_t)rhead[0] * D;
+    const T* qr1 = q + (int64_t)(seq * q_len + rq[1]) * q_stride + (int64_t)rhead[1] * D;
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+      const uint32_t lo0 = *reinterpret_cast<const uint32_t*>(qr0 + ks * 16 + quad * 2);
+      const uint32_t hi0 = *reinterpret_cast<const uint32_t*>(qr0 + ks * 16 + 8 + quad * 2);
+      const uint32_t lo1 = *reinterpret_cast<const uint32_t*>(qr1 + ks * 16 + quad * 2);
+      const uint32_t hi1 = *reinterpret_cast<const uint32_t*>(qr1 + ks * 16 + 8 + quad * 2);
+      qa[ks][0] = rok[0] ? lo0 : 0u; qa[ks][1] = rok[1] ? lo1 : 0u;
+      qa[ks][2] = rok[0] ? hi0 : 0u; qa[ks][3] = rok[1] ? hi1 : 0u;
+    }
+  } else {
     const T* qrow = q + (int64_t)seq * q_stride + (int64_t)(kvh * G + (row_ok ? row : 0)) * D;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
@@ -541,6 +593,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
 #pragma unroll
   for (int j = 0; j < NO; ++j) { o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f; }
   float m_run = -INFINITY, l_run = 0.f;         // per head row, replicated over the quad (l: this lane's share)
+  float mq_m[2] = {-INFINITY, -INFINITY}, mq_l[2] = {0.f, 0.f};   // MQ: the same for rows h = 0, 1
 
   extern __shared__ __align__(128) unsigned char dec_smem[];
   unsigned char* ring = dec_smem + (F8 ? (size_t)warp * dec_mma_smem_per_warp<TC, D>() : (size_t)warp * NST * 2 * TILE_BYTES);
@@ -601,41 +654,89 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
         mma_16816<T>(sacc[nt], qa[ks + 1], b[2], b[3]);
       }
     }
-    // ---- online softmax of head row `row` (this lane: tokens nt * 8 + quad * 2 + {0, 1})
-    float sv[4];
-    float mx = -INFINITY;
+    uint32_t pa[4];                                          // P as the A operand [16 rows x 16 tokens]
+    if constexpr (MQ) {
+      // ---- online softmax of rows r0 + row + 8 h, each masked to its own [rlo, rhi); the same operations, in the
+      // same order, as the decode path below applies to its one row
+      float sv[2][4], m_new[2];
+      bool moved = false;
 #pragma unroll
-    for (int nt = 0; nt < 2; ++nt) {
+      for (int h = 0; h < 2; ++h) {
+        float mx = -INFINITY;
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int t = base + nt * 8 + quad * 2 + e;
-        float x = sacc[nt][e] * scale2;
-        if (has_alibi) x = fmaf(slope2, (float)(t - (len - 1)), x);
-        x = (t < t1) ? x : -INFINITY;
-        sv[nt * 2 + e] = x;
-        mx = fmaxf(mx, x);
+        for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int t = base + nt * 8 + quad * 2 + e;
+            float x = sacc[nt][2 * h + e] * scale2;
+            if (has_alibi) x = fmaf(rslope[h], (float)(t - (rlen[h] - 1)), x);
+            x = (t >= rlo[h] && t < rhi[h]) ? x : -INFINITY;
+            sv[h][nt * 2 + e] = x;
+            mx = fmaxf(mx, x);
+          }
+        }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        m_new[h] = fmaxf(mq_m[h], mx);
+        moved = moved || m_new[h] > mq_m[h];
       }
-    }
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-    const float m_new = fmaxf(m_run, mx);
-    if (__any_sync(0xffffffffu, m_new > m_run)) {
-      const float corr = (m_new == -INFINITY) ? 1.f : ex2_approx(m_run - m_new);
-      l_run *= corr;
+      if (__any_sync(0xffffffffu, moved)) {
 #pragma unroll
-      for (int j = 0; j < NO; ++j) { o[j][0] *= corr; o[j][1] *= corr; }
-    }
-    m_run = m_new;
-    float pv[4];
+        for (int h = 0; h < 2; ++h) {
+          const float corr = (m_new[h] == -INFINITY) ? 1.f : ex2_approx(mq_m[h] - m_new[h]);
+          mq_l[h] *= corr;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      pv[i] = (sv[i] == -INFINITY) ? 0.f : ex2_approx(sv[i] - m_new);
-      l_run += pv[i];
+          for (int j = 0; j < NO; ++j) { o[j][2 * h] *= corr; o[j][2 * h + 1] *= corr; }
+        }
+      }
+      float pv[2][4];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mq_m[h] = m_new[h];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          pv[h][i] = (sv[h][i] == -INFINITY) ? 0.f : ex2_approx(sv[h][i] - m_new[h]);
+          mq_l[h] += pv[h][i];
+        }
+      }
+      pa[0] = pack2<T>(pv[0][0], pv[0][1]); pa[1] = pack2<T>(pv[1][0], pv[1][1]);
+      pa[2] = pack2<T>(pv[0][2], pv[0][3]); pa[3] = pack2<T>(pv[1][2], pv[1][3]);
+    } else {
+      // ---- online softmax of head row `row` (this lane: tokens nt * 8 + quad * 2 + {0, 1})
+      float sv[4];
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int t = base + nt * 8 + quad * 2 + e;
+          float x = sacc[nt][e] * scale2;
+          if (has_alibi) x = fmaf(slope2, (float)(t - (len - 1)), x);
+          x = (t < t1) ? x : -INFINITY;
+          sv[nt * 2 + e] = x;
+          mx = fmaxf(mx, x);
+        }
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run, mx);
+      if (__any_sync(0xffffffffu, m_new > m_run)) {
+        const float corr = (m_new == -INFINITY) ? 1.f : ex2_approx(m_run - m_new);
+        l_run *= corr;
+#pragma unroll
+        for (int j = 0; j < NO; ++j) { o[j][0] *= corr; o[j][1] *= corr; }
+      }
+      m_run = m_new;
+      float pv[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        pv[i] = (sv[i] == -INFINITY) ? 0.f : ex2_approx(sv[i] - m_new);
+        l_run += pv[i];
+      }
+      // a0 = tokens 0..7 of this row, a2 = tokens 8..15; rows 8..15 are zero
+      pa[0] = row_ok ? pack2<T>(pv[0], pv[1]) : 0u; pa[1] = 0u;
+      pa[2] = row_ok ? pack2<T>(pv[2], pv[3]) : 0u; pa[3] = 0u;
     }
-    // P as A operand [16 heads x 16 tokens]: a0 = tokens 0..7 of this row, a2 = tokens 8..15; rows 8..15 are zero
-    uint32_t pa[4];
-    pa[0] = row_ok ? pack2<T>(pv[0], pv[1]) : 0u; pa[1] = 0u;
-    pa[2] = row_ok ? pack2<T>(pv[2], pv[3]) : 0u; pa[3] = 0u;
     // ---- O += P V: V^T fragments through ldmatrix.trans
     {
       const int tr = (lane & 7) + ((lane >> 3) & 1) * 8;     // matrices: (tok 0..7, j), (tok 8..15, j), (0..7, j+1), (8..15, j+1)
@@ -672,6 +773,21 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
     cp_async_wait<0>();
   }
   // ---- this unit's partial result (row sum over the quad first)
+  if constexpr (MQ) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mq_l[h] += __shfl_xor_sync(0xffffffffu, mq_l[h], 1);
+      mq_l[h] += __shfl_xor_sync(0xffffffffu, mq_l[h], 2);
+      if (rok[h]) {
+        const int64_t oi = (((int64_t)(seq * q_len + rq[h]) * Hq + rhead[h]) * splits + split);
+        float* dst = o_part + oi * D + quad * 2;
+#pragma unroll
+        for (int j = 0; j < NO; ++j) *reinterpret_cast<float2*>(dst + j * 8) = make_float2(o[j][2 * h], o[j][2 * h + 1]);
+        if (quad == 0) { ml_part[oi * 2] = mq_m[h] * LN2; ml_part[oi * 2 + 1] = mq_l[h]; }
+      }
+    }
+    return;
+  }
   l_run += __shfl_xor_sync(0xffffffffu, l_run, 1);
   l_run += __shfl_xor_sync(0xffffffffu, l_run, 2);
   if (row_ok) {
@@ -681,6 +797,26 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
     for (int j = 0; j < NO; ++j) *reinterpret_cast<float2*>(dst + j * 8) = make_float2(o[j][0], o[j][1]);
     if (quad == 0) { ml_part[oi * 2] = m_run * LN2; ml_part[oi * 2 + 1] = l_run; }
   }
+}
+
+template <typename T, typename TC, int D>
+__global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
+    const T* __restrict__ q, const TC* __restrict__ k_cache, const TC* __restrict__ v_cache,
+    const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
+    float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
+    float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window) {
+  paged_mma_attend<T, TC, D, false>(q, k_cache, v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size,
+                                    max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window, 1);
+}
+
+template <typename T, typename TC, int D>
+__global__ void __launch_bounds__(DEC_THREADS, 1) paged_verify_mma_kernel(
+    const T* __restrict__ q, const TC* __restrict__ k_cache, const TC* __restrict__ v_cache,
+    const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
+    float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
+    float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window, int q_len) {
+  paged_mma_attend<T, TC, D, true>(q, k_cache, v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size,
+                                   max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window, q_len);
 }
 
 template <typename T, int D>
@@ -869,6 +1005,50 @@ int cb_paged_decode_attention(const void* q, const void* k_cache, const void* v_
 #undef DISPATCH_DEC_D
 #undef LAUNCH_DEC
 #undef LAUNCH_DEC_MMA
+  return CB_LAUNCH_CHECK();
+}
+
+// Speculative verification: q_len query tokens per sequence in one pass over the cache.  q, out: [num_seqs * q_len,
+// Hq, D], token-major (sequence i's queries are rows i * q_len + j; query j sits at position seq_lens[i] - q_len + j
+// and sees the positions before it and itself).  o_part fp32 [num_seqs * q_len, Hq, splits, D], ml_part [.., 2];
+// splits / part_len as for a decode call on num_seqs sequences (cb_decode_num_splits).  Tensor-core kernel only:
+// G <= 8, head_dim 64 / 128, 1 <= q_len <= 16.
+int cb_paged_verify_attention(const void* q, const void* k_cache, const void* v_cache, const int* block_tables,
+                              const int* seq_lens, void* out, float* o_part, float* ml_part, int num_seqs, int q_len,
+                              int Hq, int Hkv, int D, int block_size, int max_blocks_per_seq, int splits, int part_len,
+                              float scale, const float* alibi_slopes, int64_t q_stride, int64_t out_stride, int dtype,
+                              int cache_dtype, int window, cudaStream_t s) {
+  if (Hkv <= 0 || Hq % Hkv != 0 || Hq / Hkv > MAX_GROUP || (D != 64 && D != 128) || q_len < 1 || q_len > 16)
+    return (int)cudaErrorInvalidValue;
+  if (cache_dtype != dtype && cache_dtype != CB_F8E5M2) return (int)cudaErrorInvalidValue;
+  if (num_seqs == 0) return 0;
+  const int units = Hkv * ((q_len * (Hq / Hkv) + 15) / 16);        // (kv head, 16-row slice) pairs = warps needed
+  const int warps = units < DEC_THREADS / 32 ? units : DEC_THREADS / 32;
+  const dim3 grid(num_seqs, (units + warps - 1) / warps, splits);
+#define LAUNCH_VERIFY(T, TC, DD)                                                                                    \
+  {                                                                                                                  \
+    constexpr int per_warp = dec_mma_smem_per_warp<TC, DD>();                                                        \
+    static bool attr_done = false;                                                                                   \
+    if (!attr_done) {                                                                                                \
+      cudaFuncSetAttribute(paged_verify_mma_kernel<T, TC, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
+                           (DEC_THREADS / 32) * per_warp);                                                           \
+      attr_done = true;                                                                                              \
+    }                                                                                                                \
+    paged_verify_mma_kernel<T, TC, DD><<<grid, warps * 32, warps * per_warp, s>>>(                                   \
+        (const T*)q, (const TC*)k_cache, (const TC*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv,      \
+        block_size, max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window, q_len);            \
+    decode_reduce_kernel<T, DD><<<dim3(num_seqs * q_len, Hq), 128, 0, s>>>(o_part, ml_part, (T*)out, Hq, splits,     \
+                                                                          out_stride);                               \
+  }
+#define DISPATCH_VERIFY_D(T, TC)                                                                                    \
+  if (D == 128) { LAUNCH_VERIFY(T, TC, 128); }                                                                       \
+  else { LAUNCH_VERIFY(T, TC, 64); }
+  CB_DISPATCH_HALF(dtype, T, {
+    if (cache_dtype == CB_F8E5M2) { DISPATCH_VERIFY_D(T, __nv_fp8_e5m2) }
+    else { DISPATCH_VERIFY_D(T, T) }
+  });
+#undef DISPATCH_VERIFY_D
+#undef LAUNCH_VERIFY
   return CB_LAUNCH_CHECK();
 }
 

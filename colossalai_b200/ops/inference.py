@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes
 import math
+import os
 from typing import Optional, Tuple
 
 import torch
@@ -92,10 +93,16 @@ def _decode_workspace(q: torch.Tensor, n: int, heads: int, splits: int, head_dim
 
 def paged_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_tables: torch.Tensor,
                            seq_lens: torch.Tensor, scale: Optional[float] = None,
-                           alibi_slopes: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
-    """q: [num_seqs, Hq, D] (one new token per sequence) -> [num_seqs, Hq, D].  `window`: sliding-window attention
-    (only the last `window` cached tokens are visible), handled inside the split-KV kernel (`window_start`).  An fp8
-    (uint8) cache is decoded exactly to the query dtype inside the kernel."""
+                           alibi_slopes: Optional[torch.Tensor] = None, window: Optional[int] = None,
+                           q_len: int = 1) -> torch.Tensor:
+    """q: [num_seqs * q_len, Hq, D] -> same shape.  `seq_lens` [num_seqs] counts the cached tokens including the
+    step's; sequence i's queries are rows i * q_len + j (token-major), and query j sits at position
+    seq_lens[i] - q_len + j and sees the positions up to its own.  q_len = 1 is a decode step, q_len > 1 the
+    speculative verification of q_len - 1 drafted tokens (one pass over the cache).  `window`: sliding-window attention
+    (only the last `window` positions a query sees are visible), handled inside the split-KV kernel (`window_start`).
+    An fp8 (uint8) cache is decoded exactly to the query dtype inside the kernel."""
+    if q_len != 1:
+        return _paged_verify_attention(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window, q_len)
     n, Hq, D = q.shape
     nb, bs, Hkv, _ = k_cache.shape
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
@@ -124,17 +131,59 @@ def paged_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torc
     return paged_decode_attention_ref(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window)
 
 
+def _paged_verify_attention(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window, q_len):
+    """`paged_decode_attention` with q_len query tokens per sequence: one tensor-core pass where the kernel covers the
+    shape, one decode call per query position where only the CUDA-core kernel does (head_dim 256,
+    CB200_DECODE=simt), the reference elsewhere."""
+    rows, Hq, D = q.shape
+    nb, bs, Hkv, _ = k_cache.shape
+    assert q_len >= 1 and rows % q_len == 0, (rows, q_len)
+    n = rows // q_len
+    scale = scale if scale is not None else 1.0 / math.sqrt(D)
+    native = (use_native(q) and q.dtype in (torch.float16, torch.bfloat16)
+              and k_cache.dtype in (q.dtype, FP8_CACHE_DTYPE) and Hq // Hkv <= 8)
+    simt = os.environ.get("CB200_DECODE", "").startswith("s")
+    if native and D in (64, 128) and q_len <= 16 and not simt:
+        lib = _get_lib()
+        part = ctypes.c_int(0)
+        splits = lib.cb_decode_num_splits(n, Hkv, block_tables.shape[1] * bs, ctypes.byref(part))
+        out = torch.empty_like(q)
+        ws = _decode_workspace(q, rows, Hq, splits, D)
+        if ws is not None:
+            o_part, ml_part = ws
+        else:
+            o_part = torch.empty(rows, Hq, splits, D, dtype=torch.float32, device=q.device)
+            ml_part = torch.empty(rows, Hq, splits, 2, dtype=torch.float32, device=q.device)
+        qc = q if q.stride(2) == 1 and q.stride(1) == D else q.contiguous()
+        loader.check(lib.cb_paged_verify_attention(
+            loader.ptr(qc), loader.ptr(k_cache), loader.ptr(v_cache), loader.ptr(block_tables), loader.ptr(seq_lens),
+            loader.ptr(out), loader.ptr(o_part), loader.ptr(ml_part), n, q_len, Hq, Hkv, D, bs, block_tables.shape[1],
+            splits, part.value, ctypes.c_float(scale), loader.ptr(alibi_slopes), ctypes.c_int64(qc.stride(0)),
+            ctypes.c_int64(out.stride(0)), code(q.dtype), _cache_code(k_cache), int(window or 0),
+            loader.stream_ptr()),
+            "paged_decode_attention")
+        loader.launch_counter.add("paged_decode_attention", 2)
+        return out
+    if native and D in (64, 128, 256):
+        qs = q.view(n, q_len, Hq, D)
+        outs = [paged_decode_attention(qs[:, j], k_cache, v_cache, block_tables, seq_lens - (q_len - 1 - j), scale,
+                                       alibi_slopes, window) for j in range(q_len)]
+        return torch.stack(outs, 1).view(rows, Hq, D)
+    return paged_decode_attention_ref(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window, q_len)
+
+
 def paged_decode_attention_ref(q, k_cache, v_cache, block_tables, seq_lens, scale=None, alibi_slopes=None,
-                               window=None):
-    n, Hq, D = q.shape
+                               window=None, q_len=1):
+    rows, Hq, D = q.shape
     nb, bs, Hkv, _ = k_cache.shape
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     G = Hq // Hkv
     out = torch.empty_like(q)
-    for i in range(n):
-        L = int(seq_lens[i])
-        k = gather_paged_kv(k_cache, block_tables[i], L, torch.float32)
-        v = gather_paged_kv(v_cache, block_tables[i], L, torch.float32)
+    for i in range(rows):
+        s_i = i // q_len                              # sequence of row i; its query sees L positions
+        L = int(seq_lens[s_i]) - (q_len - 1 - i % q_len)
+        k = gather_paged_kv(k_cache, block_tables[s_i], L, torch.float32)
+        v = gather_paged_kv(v_cache, block_tables[s_i], L, torch.float32)
         if window is not None and L > window:
             k, v, L = k[L - window:], v[L - window:], window
         k = k.repeat_interleave(G, dim=1)
