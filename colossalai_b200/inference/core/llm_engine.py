@@ -136,24 +136,19 @@ class LLMEngine(BaseEngine):
         per sequence (speculative verification) need that many rows of partials per sequence."""
         if not torch.cuda.is_available() or not k_caches or k_caches[0].device.type != "cuda":
             return
-        import ctypes
-
         from ...ops import inference as infer_ops
         from ..flash_decoding_utils import FDIntermTensors
 
         cfg = self.inference_config
+        device = k_caches[0].device
         hkv, d = k_caches[0].shape[2], k_caches[0].shape[3]
         hq = hkv * (self.model_config.num_attention_heads // max(self.model_config.num_key_value_heads, 1))
         max_len = cfg.max_input_len + cfg.max_output_len
         max_len = (max_len + cfg.block_size - 1) // cfg.block_size * cfg.block_size
-        try:
-            lib = infer_ops._get_lib()
-            part = ctypes.c_int(0)
-            worst = max(n * q_per_seq * lib.cb_decode_num_splits(n, hkv, max_len, ctypes.byref(part))
-                        for n in range(1, cfg.max_batch_size + 1))
-            FDIntermTensors().ensure(worst, hq, d, device=k_caches[0].device)
-        except Exception as e:                # extension not built / odd config: the op allocates per call instead
-            self.logger.warning(f"persistent decode workspace disabled: {e}", ranks=[0])
+        sms = infer_ops.sm_count(device.index)
+        worst = max(n * q_per_seq * infer_ops.decode_splits(n, hkv, max_len, sms)[0]
+                    for n in range(1, cfg.max_batch_size + 1))
+        FDIntermTensors().ensure(worst, hq, d, device=device)
 
     def _model_forward(self, input_ids: torch.Tensor, positions: torch.Tensor) -> torch.Tensor:
         """input_ids: flattened tokens [T]; returns hidden->logits of the LAST token of every sequence."""

@@ -6,17 +6,16 @@
 //   cb_kv_cache_write        : scatter this step's K,V rows [tokens, kv_heads, D] into their paged slots (prefill: all
 //                              prompt tokens via cu_seqlens; decode: one token per sequence); a 16-bit cache stores the
 //                              rows as they are, an fp8 cache (uint8 bytes) stores them rounded to e5m2
-//   cb_rope_kv_cache_write   : fused RoPE(q,k) in place + cache write of rotated K and of V (decode path)
 //   cb_paged_decode_attention: split-KV flash-decoding: grid (seq, group of <= 8 kv heads, split); one WARP serves a
 //                              kv head (its whole GQA group, so K/V are read once per group) and the warps of a CTA
 //                              stream adjacent head slices of the same token rows; fp32 online softmax; second pass
 //                              merges splits; an e5m2 cache is decoded exactly to the query dtype after the load, so
-//                              the result is bitwise that of the 16-bit cache holding the decoded values
-//   cb_paged_verify_attention: the same split-KV pass for q_len <= 16 query tokens per sequence (speculative
-//                              verification): the MMA rows are (query token, q head) pairs, so up to 16 / G tokens cost
-//                              one decode pass over K/V; each token sees the cache up to its own position, and without a
-//                              window each output row is bitwise the decode kernel's result for that token alone
-//   cb_gather_cos_sin        : per-token cos/sin rows from the [max_pos, D/2] caches
+//                              the result is bitwise that of the 16-bit cache holding the decoded values.  Head_dim
+//                              64 / 128 run on tensor cores, head_dim 256 on CUDA cores.  At head_dim 64 / 128 the
+//                              same pass takes q_len <= 16 query tokens per sequence (speculative verification): the
+//                              MMA rows are (query token, q head) pairs, so up to 16 / G tokens cost one decode pass
+//                              over K/V; each token sees the cache up to its own position, and without a window each
+//                              output row is bitwise the single-token result for that token alone
 //   cb_convert_fp8           : fp16/bf16/fp32 <-> fp8 e5m2 storage
 //
 // Capability parity: reference inference_ops_cuda (extensions/csrc/kernel/cuda/{flash_decoding_attention,
@@ -105,43 +104,6 @@ __global__ void __launch_bounds__(256) kv_cache_write_kernel(const T* __restrict
   }
 }
 
-// RoPE (half rotation) on q [tokens, Hq, D] and k [tokens, Hkv, D] in place, then K,V -> paged cache.
-template <typename T>
-__global__ void __launch_bounds__(256) rope_kv_cache_write_kernel(T* __restrict__ q, T* __restrict__ k,
-                                                                  const T* __restrict__ v, T* __restrict__ k_cache,
-                                                                  T* __restrict__ v_cache,
-                                                                  const float* __restrict__ cos_c,
-                                                                  const float* __restrict__ sin_c,
-                                                                  const int* __restrict__ block_tables,
-                                                                  const int* __restrict__ token_seq,
-                                                                  const int* __restrict__ token_pos, int tokens, int Hq,
-                                                                  int Hkv, int D, int rot, int block_size,
-                                                                  int max_blocks_per_seq, int64_t q_stride,
-                                                                  int64_t k_stride, int64_t v_stride) {
-  const int t = blockIdx.x;
-  if (t >= tokens) return;
-  const int seq = token_seq[t], pos = token_pos[t];
-  const int half = rot / 2;
-  const float* cp = cos_c + (int64_t)pos * half;
-  const float* sp = sin_c + (int64_t)pos * half;
-  T* qt = q + (int64_t)t * q_stride;
-  T* kt = k + (int64_t)t * k_stride;
-  for (int i = threadIdx.x; i < (Hq + Hkv) * half; i += blockDim.x) {
-    const int h = i / half, j = i - h * half;
-    T* base = h < Hq ? qt + h * D : kt + (h - Hq) * D;
-    const float a = to_f32<T>(base[j]), b = to_f32<T>(base[j + half]), c = cp[j], s = sp[j];
-    base[j] = from_f32<T>(a * c - b * s);
-    base[j + half] = from_f32<T>(b * c + a * s);
-  }
-  __syncthreads();
-  const int blk = block_tables[seq * max_blocks_per_seq + pos / block_size];
-  const int64_t dst = ((int64_t)blk * block_size + pos % block_size) * Hkv * D;
-  for (int i = threadIdx.x; i < Hkv * D; i += blockDim.x) {
-    k_cache[dst + i] = kt[i];
-    v_cache[dst + i] = v[(int64_t)t * v_stride + i];
-  }
-}
-
 // 16-byte vectorised variants (the hot ones): one thread moves one 16-byte vector, grid = all vectors of the step, so a
 // prefill of thousands of tokens is a single HBM-rate streaming kernel instead of one small CTA per token.  An e5m2
 // cache (TC = __nv_fp8_e5m2) takes the same 16 input bytes per thread and stores 8.
@@ -167,60 +129,6 @@ __global__ void __launch_bounds__(256) kv_cache_write_vec_kernel(const T* __rest
                            : __ldg(reinterpret_cast<const uint4*>(k + (int64_t)t * k_stride) + i);
     if constexpr (sizeof(TC) == 1) reinterpret_cast<uint2*>(is_v ? v_cache : k_cache)[dst] = e5m2_pack8<T>(val);
     else reinterpret_cast<uint4*>(is_v ? v_cache : k_cache)[dst] = val;
-  }
-}
-
-// RoPE (half rotation, rot == D) on q and k in place + rotated K and V into the paged cache, 16-byte vectors: a work
-// item is one (token, head, 8-element group of the FIRST half) - it owns the matching group of the second half too -
-// or one V vector.  K is written to the cache from registers (no second pass, no block barrier).
-template <typename T>
-__global__ void __launch_bounds__(256) rope_kv_cache_write_vec_kernel(
-    T* __restrict__ q, T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache, T* __restrict__ v_cache,
-    const float* __restrict__ cos_c, const float* __restrict__ sin_c, const int* __restrict__ block_tables,
-    const int* __restrict__ token_seq, const int* __restrict__ token_pos, int tokens, int Hq, int Hkv, int D,
-    int block_size, int max_blocks_per_seq, int64_t q_stride, int64_t k_stride, int64_t v_stride) {
-  const int half = D / 2;
-  const int gph = half / 8;                          // 8-element groups per half head
-  const int rope_items = (Hq + Hkv) * gph;
-  const int v_items = Hkv * D / 8;
-  const int per_tok = rope_items + v_items;
-  const int64_t total = (int64_t)tokens * per_tok;
-  for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total; w += (int64_t)gridDim.x * blockDim.x) {
-    const int t = (int)(w / per_tok);
-    const int r = (int)(w - (int64_t)t * per_tok);
-    const int seq = __ldg(token_seq + t), pos = __ldg(token_pos + t);
-    const int blk = __ldg(block_tables + seq * max_blocks_per_seq + pos / block_size);
-    const int64_t slot = ((int64_t)blk * block_size + pos % block_size) * Hkv * D;              // in elements
-    if (r >= rope_items) {
-      const int i = r - rope_items;
-      reinterpret_cast<uint4*>(v_cache + slot)[i] = __ldg(reinterpret_cast<const uint4*>(v + (int64_t)t * v_stride) + i);
-      continue;
-    }
-    const int h = r / gph, g = r - h * gph;
-    T* base = h < Hq ? q + (int64_t)t * q_stride + (int64_t)h * D : k + (int64_t)t * k_stride + (int64_t)(h - Hq) * D;
-    Vec16<T> a, b2;
-    a.load(base + g * 8);
-    b2.load(base + half + g * 8);
-    const float4 c0 = __ldg(reinterpret_cast<const float4*>(cos_c + (int64_t)pos * half + g * 8));
-    const float4 c1 = __ldg(reinterpret_cast<const float4*>(cos_c + (int64_t)pos * half + g * 8 + 4));
-    const float4 s0 = __ldg(reinterpret_cast<const float4*>(sin_c + (int64_t)pos * half + g * 8));
-    const float4 s1 = __ldg(reinterpret_cast<const float4*>(sin_c + (int64_t)pos * half + g * 8 + 4));
-    const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-    const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-    Vec16<T> oa, ob;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float x = a.get(e), y = b2.get(e);
-      oa.set(e, x * cs[e] - y * sn[e]);
-      ob.set(e, y * cs[e] + x * sn[e]);
-    }
-    oa.store(base + g * 8);
-    ob.store(base + half + g * 8);
-    if (h >= Hq) {
-      T* kc = k_cache + slot + (int64_t)(h - Hq) * D;
-      oa.store(kc + g * 8);
-      ob.store(kc + half + g * 8);
-    }
   }
 }
 
@@ -443,7 +351,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_kernel(
 }
 
 // ----------------------------------------------------------------------------------------------------------------
-// Tensor-core formulation of the same split-KV decode step (the default; `CB200_DECODE=simt` selects the kernel above).
+// Tensor-core formulation of the same split-KV decode step (head_dim 64 / 128; the kernel above serves head_dim 256).
 //
 // The CUDA-core kernel above executes ~89 warp-instructions per (token, kv head) - two FMAs per cached element and q
 // head - which is as much issue time as the HBM transfer takes (ncu: 93 M warp-instructions, 45 % issue-active,
@@ -799,24 +707,16 @@ CB_DEVICE void paged_mma_attend(
   }
 }
 
-template <typename T, typename TC, int D>
-__global__ void __launch_bounds__(DEC_THREADS, 1) paged_decode_mma_kernel(
-    const T* __restrict__ q, const TC* __restrict__ k_cache, const TC* __restrict__ v_cache,
-    const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
-    float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
-    float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window) {
-  paged_mma_attend<T, TC, D, false>(q, k_cache, v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size,
-                                    max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window, 1);
-}
-
-template <typename T, typename TC, int D>
-__global__ void __launch_bounds__(DEC_THREADS, 1) paged_verify_mma_kernel(
+// MQ = false ignores q_len: the decode instantiation is compiled for exactly one query token per sequence.
+template <typename T, typename TC, int D, bool MQ>
+__global__ void __launch_bounds__(DEC_THREADS, 1) paged_mma_kernel(
     const T* __restrict__ q, const TC* __restrict__ k_cache, const TC* __restrict__ v_cache,
     const int* __restrict__ block_tables, const int* __restrict__ seq_lens, float* __restrict__ o_part,
     float* __restrict__ ml_part, int Hq, int Hkv, int block_size, int max_blocks_per_seq, int splits, int part_len,
     float scale, const float* __restrict__ alibi_slopes, int64_t q_stride, int window, int q_len) {
-  paged_mma_attend<T, TC, D, true>(q, k_cache, v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size,
-                                   max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window, q_len);
+  paged_mma_attend<T, TC, D, MQ>(q, k_cache, v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size,
+                                 max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window,
+                                 MQ ? q_len : 1);
 }
 
 template <typename T, int D>
@@ -843,20 +743,70 @@ __global__ void __launch_bounds__(128) decode_reduce_kernel(const float* __restr
   }
 }
 
-__global__ void gather_cos_sin_kernel(const float* __restrict__ cos_c, const float* __restrict__ sin_c,
-                                      const int* __restrict__ pos, float* __restrict__ cos_o,
-                                      float* __restrict__ sin_o, int tokens, int half) {
-  const int t = blockIdx.x;
-  for (int i = threadIdx.x; i < half; i += blockDim.x) {
-    cos_o[(int64_t)t * half + i] = cos_c[(int64_t)pos[t] * half + i];
-    sin_o[(int64_t)t * half + i] = sin_c[(int64_t)pos[t] * half + i];
-  }
-}
-
 template <typename TI, typename TO>
 __global__ void convert_kernel(const TI* __restrict__ in, TO* __restrict__ out, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = (TO)(float)in[i];
+}
+
+// cb_paged_decode_attention's arguments, shared by the launchers below
+struct PagedArgs {
+  const void *q, *k_cache, *v_cache;
+  const int *block_tables, *seq_lens;
+  void* out;
+  float *o_part, *ml_part;
+  int num_seqs, q_len, Hq, Hkv, block_size, max_blocks_per_seq, splits, part_len;
+  float scale;
+  const float* alibi_slopes;
+  int64_t q_stride, out_stride;
+  int window;
+  cudaStream_t s;
+};
+
+// Tensor-core split-KV pass, then the reduce: one warp per (kv head, 16-row slice of its q_len x G rows).
+template <typename T, typename TC, int D, bool MQ> void launch_paged_mma(const PagedArgs& a) {
+  constexpr int per_warp = dec_mma_smem_per_warp<TC, D>();
+  static bool attr_done = false;
+  if (!attr_done) {
+    cudaFuncSetAttribute(paged_mma_kernel<T, TC, D, MQ>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (DEC_THREADS / 32) * per_warp);
+    attr_done = true;
+  }
+  const int units = a.Hkv * ((a.q_len * (a.Hq / a.Hkv) + 15) / 16);
+  const int warps = units < DEC_THREADS / 32 ? units : DEC_THREADS / 32;
+  paged_mma_kernel<T, TC, D, MQ><<<dim3(a.num_seqs, (units + warps - 1) / warps, a.splits), warps * 32,
+                                   warps * per_warp, a.s>>>(
+      (const T*)a.q, (const TC*)a.k_cache, (const TC*)a.v_cache, a.block_tables, a.seq_lens, a.o_part, a.ml_part, a.Hq,
+      a.Hkv, a.block_size, a.max_blocks_per_seq, a.splits, a.part_len, a.scale, a.alibi_slopes, a.q_stride, a.window,
+      a.q_len);
+  decode_reduce_kernel<T, D><<<dim3(a.num_seqs * a.q_len, a.Hq), 128, 0, a.s>>>(a.o_part, a.ml_part, (T*)a.out, a.Hq,
+                                                                               a.splits, a.out_stride);
+}
+
+// CUDA-core split-KV pass at head_dim 256 (one query token per sequence), then the reduce: one warp per (kv head,
+// set of <= 4 q heads).
+template <typename T, typename TC> void launch_paged_cuda_core(const PagedArgs& a) {
+  constexpr int ring_bytes = DEC_STAGES * (2 * DEC_U * 2 * 32) * 16;                  // per-warp cp.async ring
+  static bool attr_done = false;
+  if (!attr_done) {
+    cudaFuncSetAttribute(paged_decode_kernel<T, TC, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (DEC_THREADS / 32) * ring_bytes);
+    attr_done = true;
+  }
+  const int units = a.Hkv * ((a.Hq / a.Hkv + DEC_GH - 1) / DEC_GH);
+  const int warps = units < DEC_THREADS / 32 ? units : DEC_THREADS / 32;
+  paged_decode_kernel<T, TC, 256><<<dim3(a.num_seqs, (units + warps - 1) / warps, a.splits), warps * 32,
+                                    warps * ring_bytes, a.s>>>(
+      (const T*)a.q, (const TC*)a.k_cache, (const TC*)a.v_cache, a.block_tables, a.seq_lens, a.o_part, a.ml_part, a.Hq,
+      a.Hkv, a.block_size, a.max_blocks_per_seq, a.splits, a.part_len, a.scale, a.alibi_slopes, a.q_stride, a.window);
+  decode_reduce_kernel<T, 256><<<dim3(a.num_seqs, a.Hq), 128, 0, a.s>>>(a.o_part, a.ml_part, (T*)a.out, a.Hq, a.splits,
+                                                                        a.out_stride);
+}
+
+template <typename T, typename TC> void launch_paged(const PagedArgs& a, int D) {
+  if (D == 256) launch_paged_cuda_core<T, TC>(a);
+  else if (D == 128) a.q_len == 1 ? launch_paged_mma<T, TC, 128, false>(a) : launch_paged_mma<T, TC, 128, true>(a);
+  else a.q_len == 1 ? launch_paged_mma<T, TC, 64, false>(a) : launch_paged_mma<T, TC, 64, true>(a);
 }
 
 }  // namespace
@@ -900,162 +850,30 @@ int cb_kv_cache_write(const void* k, const void* v, void* k_cache, void* v_cache
   return CB_LAUNCH_CHECK();
 }
 
-int cb_rope_kv_cache_write(void* q, void* k, const void* v, void* k_cache, void* v_cache, const float* cos_c,
-                           const float* sin_c, const int* block_tables, const int* token_seq, const int* token_pos,
-                           int tokens, int Hq, int Hkv, int D, int rot, int block_size, int max_blocks_per_seq,
-                           int64_t q_stride, int64_t k_stride, int64_t v_stride, int dtype, cudaStream_t s) {
-  if (tokens == 0) return 0;
-  if (rot == D && D % 16 == 0 && q_stride % 8 == 0 && k_stride % 8 == 0 && v_stride % 8 == 0 &&
-      ((uintptr_t)q % 16) == 0 && ((uintptr_t)k % 16) == 0 && ((uintptr_t)v % 16) == 0 &&
-      ((uintptr_t)k_cache % 16) == 0 && ((uintptr_t)v_cache % 16) == 0 && ((uintptr_t)cos_c % 16) == 0 &&
-      ((uintptr_t)sin_c % 16) == 0) {
-    const int64_t total = (int64_t)tokens * ((Hq + Hkv) * (D / 16) + Hkv * D / 8);
-    const int grid = (int)((total + 255) / 256 < 16 * cb_num_sms() ? (total + 255) / 256 : 16 * cb_num_sms());
-    CB_DISPATCH_HALF(dtype, T, {
-      rope_kv_cache_write_vec_kernel<T><<<grid, 256, 0, s>>>((T*)q, (T*)k, (const T*)v, (T*)k_cache, (T*)v_cache, cos_c,
-                                                            sin_c, block_tables, token_seq, token_pos, tokens, Hq, Hkv, D,
-                                                            block_size, max_blocks_per_seq, q_stride, k_stride, v_stride);
-    });
-    return CB_LAUNCH_CHECK();
-  }
-  CB_DISPATCH_HALF(dtype, T, {
-    rope_kv_cache_write_kernel<T><<<tokens, 256, 0, s>>>((T*)q, (T*)k, (const T*)v, (T*)k_cache, (T*)v_cache, cos_c,
-                                                        sin_c, block_tables, token_seq, token_pos, tokens, Hq, Hkv, D,
-                                                        rot, block_size, max_blocks_per_seq, q_stride, k_stride,
-                                                        v_stride);
-  });
-  return CB_LAUNCH_CHECK();
-}
-
-int cb_decode_num_splits(int num_seqs, int kv_heads, int max_len, int* part_len_out) {
-  // one CTA (up to 8 warps, one per kv head) per SM: aim at >= 2 waves of CTAs, partitions of >= 64 tokens
-  const int ctas_per_split = num_seqs * ((kv_heads + 7) / 8);
-  const int target = 2 * cb_num_sms();
-  int splits = (target + ctas_per_split - 1) / ctas_per_split;
-  const int max_splits = (max_len + 63) / 64;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  int part = (max_len + splits - 1) / splits;
-  part = ((part + 31) / 32) * 32;
-  splits = (max_len + part - 1) / part;
-  if (splits < 1) splits = 1;
-  *part_len_out = part;
-  return splits;
-}
-
-// q: [num_seqs, Hq, D] of `dtype`; out same; caches [nb, bs, Hkv, D] of `cache_dtype` (`dtype` or CB_F8E5M2);
-// o_part fp32 [num_seqs, Hq, splits, D]; ml_part [.., 2]
+// Paged attention for q_len query tokens per sequence.  q, out: [num_seqs * q_len, Hq, D] of `dtype`, token-major
+// (sequence i's queries are rows i * q_len + j; query j sits at position seq_lens[i] - q_len + j and sees the positions
+// before it and itself); caches [nb, bs, Hkv, D] of `cache_dtype` (`dtype` or CB_F8E5M2); o_part fp32
+// [num_seqs * q_len, Hq, splits, D], ml_part [.., 2]; splits / part_len as `ops/inference.py` `decode_splits` gives
+// them for num_seqs sequences, whatever q_len.  Served: G = Hq / Hkv <= 8 with head_dim 64 / 128 and
+// 1 <= q_len <= 16 (tensor cores), or head_dim 256 and q_len = 1 (CUDA cores); anything else launches nothing and
+// returns cudaErrorInvalidValue.
 int cb_paged_decode_attention(const void* q, const void* k_cache, const void* v_cache, const int* block_tables,
-                              const int* seq_lens, void* out, float* o_part, float* ml_part, int num_seqs, int Hq,
-                              int Hkv, int D, int block_size, int max_blocks_per_seq, int splits, int part_len,
-                              float scale, const float* alibi_slopes, int64_t q_stride, int64_t out_stride, int dtype,
-                              int cache_dtype, int window, cudaStream_t s) {
-  if (num_seqs == 0) return 0;
-  if (Hq % Hkv != 0 || Hq / Hkv > MAX_GROUP) return (int)cudaErrorInvalidValue;
-  if (cache_dtype != dtype && cache_dtype != CB_F8E5M2) return (int)cudaErrorInvalidValue;
-  const int G = Hq / Hkv;
-  const int units = Hkv * ((G + DEC_GH - 1) / DEC_GH);             // (kv head, query-head set) pairs = warps needed
-  const int warps = units < DEC_THREADS / 32 ? units : DEC_THREADS / 32;
-  dim3 grid(num_seqs, (units + warps - 1) / warps, splits);
-  const int dec_smem = warps * DEC_STAGES * (2 * DEC_U * 2 * 32) * 16;                    // per-warp cp.async rings
-  constexpr int dec_smem_max = (DEC_THREADS / 32) * DEC_STAGES * (2 * DEC_U * 2 * 32) * 16;
-  // default: the tensor-core formulation (mma.sync over the GQA group) where it applies (head_dim 64 / 128, groups of
-  // <= 8 q heads); CB200_DECODE=simt forces the CUDA-core kernel (also used for head_dim 256)
-  const char* impl_env = getenv("CB200_DECODE");
-  const bool use_mma = !(impl_env != nullptr && impl_env[0] == 's') && G <= 8 && (D == 128 || D == 64);
-  const int mma_warps = Hkv < DEC_THREADS / 32 ? Hkv : DEC_THREADS / 32;
-  dim3 mma_grid(num_seqs, (Hkv + mma_warps - 1) / mma_warps, splits);
-#define LAUNCH_DEC_MMA(T, TC, DD)                                                                                   \
-  {                                                                                                                  \
-    constexpr int per_warp = dec_mma_smem_per_warp<TC, DD>();                                                        \
-    static bool attr_done = false;                                                                                   \
-    if (!attr_done) {                                                                                                \
-      cudaFuncSetAttribute(paged_decode_mma_kernel<T, TC, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
-                           (DEC_THREADS / 32) * per_warp);                                                           \
-      attr_done = true;                                                                                              \
-    }                                                                                                                \
-    paged_decode_mma_kernel<T, TC, DD><<<mma_grid, mma_warps * 32, mma_warps * per_warp, s>>>(                       \
-        (const T*)q, (const TC*)k_cache, (const TC*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv,      \
-        block_size, max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window);                   \
-    decode_reduce_kernel<T, DD><<<dim3(num_seqs, Hq), 128, 0, s>>>(o_part, ml_part, (T*)out, Hq, splits, out_stride); \
-  }
-#define LAUNCH_DEC(T, TC, DD)                                                                                       \
-  {                                                                                                                  \
-    static bool attr_done = false;                                                                                   \
-    if (!attr_done) {                                                                                                \
-      cudaFuncSetAttribute(paged_decode_kernel<T, TC, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, dec_smem_max);\
-      attr_done = true;                                                                                              \
-    }                                                                                                                \
-  }                                                                                                                  \
-  paged_decode_kernel<T, TC, DD><<<grid, warps * 32, dec_smem, s>>>((const T*)q, (const TC*)k_cache,                 \
-      (const TC*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv, block_size, max_blocks_per_seq, splits,  \
-      part_len, scale, alibi_slopes, q_stride, window);                                                              \
-  decode_reduce_kernel<T, DD><<<dim3(num_seqs, Hq), 128, 0, s>>>(o_part, ml_part, (T*)out, Hq, splits, out_stride)
-#define DISPATCH_DEC_D(T, TC)                                                                                       \
-  if (use_mma && D == 128) { LAUNCH_DEC_MMA(T, TC, 128); }                                                           \
-  else if (use_mma && D == 64) { LAUNCH_DEC_MMA(T, TC, 64); }                                                        \
-  else if (D == 128) { LAUNCH_DEC(T, TC, 128); }                                                                     \
-  else if (D == 64) { LAUNCH_DEC(T, TC, 64); }                                                                       \
-  else if (D == 256) { LAUNCH_DEC(T, TC, 256); }                                                                     \
-  else return (int)cudaErrorInvalidValue;
-  CB_DISPATCH_HALF(dtype, T, {
-    if (cache_dtype == CB_F8E5M2) { DISPATCH_DEC_D(T, __nv_fp8_e5m2) }
-    else { DISPATCH_DEC_D(T, T) }
-  });
-#undef DISPATCH_DEC_D
-#undef LAUNCH_DEC
-#undef LAUNCH_DEC_MMA
-  return CB_LAUNCH_CHECK();
-}
-
-// Speculative verification: q_len query tokens per sequence in one pass over the cache.  q, out: [num_seqs * q_len,
-// Hq, D], token-major (sequence i's queries are rows i * q_len + j; query j sits at position seq_lens[i] - q_len + j
-// and sees the positions before it and itself).  o_part fp32 [num_seqs * q_len, Hq, splits, D], ml_part [.., 2];
-// splits / part_len as for a decode call on num_seqs sequences (cb_decode_num_splits).  Tensor-core kernel only:
-// G <= 8, head_dim 64 / 128, 1 <= q_len <= 16.
-int cb_paged_verify_attention(const void* q, const void* k_cache, const void* v_cache, const int* block_tables,
                               const int* seq_lens, void* out, float* o_part, float* ml_part, int num_seqs, int q_len,
                               int Hq, int Hkv, int D, int block_size, int max_blocks_per_seq, int splits, int part_len,
                               float scale, const float* alibi_slopes, int64_t q_stride, int64_t out_stride, int dtype,
                               int cache_dtype, int window, cudaStream_t s) {
-  if (Hkv <= 0 || Hq % Hkv != 0 || Hq / Hkv > MAX_GROUP || (D != 64 && D != 128) || q_len < 1 || q_len > 16)
+  const int max_q_len = (D == 64 || D == 128) ? 16 : D == 256 ? 1 : 0;
+  if (Hkv <= 0 || Hq % Hkv != 0 || Hq / Hkv > MAX_GROUP || q_len < 1 || q_len > max_q_len)
     return (int)cudaErrorInvalidValue;
   if (cache_dtype != dtype && cache_dtype != CB_F8E5M2) return (int)cudaErrorInvalidValue;
   if (num_seqs == 0) return 0;
-  const int units = Hkv * ((q_len * (Hq / Hkv) + 15) / 16);        // (kv head, 16-row slice) pairs = warps needed
-  const int warps = units < DEC_THREADS / 32 ? units : DEC_THREADS / 32;
-  const dim3 grid(num_seqs, (units + warps - 1) / warps, splits);
-#define LAUNCH_VERIFY(T, TC, DD)                                                                                    \
-  {                                                                                                                  \
-    constexpr int per_warp = dec_mma_smem_per_warp<TC, DD>();                                                        \
-    static bool attr_done = false;                                                                                   \
-    if (!attr_done) {                                                                                                \
-      cudaFuncSetAttribute(paged_verify_mma_kernel<T, TC, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
-                           (DEC_THREADS / 32) * per_warp);                                                           \
-      attr_done = true;                                                                                              \
-    }                                                                                                                \
-    paged_verify_mma_kernel<T, TC, DD><<<grid, warps * 32, warps * per_warp, s>>>(                                   \
-        (const T*)q, (const TC*)k_cache, (const TC*)v_cache, block_tables, seq_lens, o_part, ml_part, Hq, Hkv,      \
-        block_size, max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, window, q_len);            \
-    decode_reduce_kernel<T, DD><<<dim3(num_seqs * q_len, Hq), 128, 0, s>>>(o_part, ml_part, (T*)out, Hq, splits,     \
-                                                                          out_stride);                               \
-  }
-#define DISPATCH_VERIFY_D(T, TC)                                                                                    \
-  if (D == 128) { LAUNCH_VERIFY(T, TC, 128); }                                                                       \
-  else { LAUNCH_VERIFY(T, TC, 64); }
+  const PagedArgs a{q, k_cache, v_cache, block_tables, seq_lens, out, o_part, ml_part, num_seqs, q_len, Hq, Hkv,
+                    block_size, max_blocks_per_seq, splits, part_len, scale, alibi_slopes, q_stride, out_stride,
+                    window, s};
   CB_DISPATCH_HALF(dtype, T, {
-    if (cache_dtype == CB_F8E5M2) { DISPATCH_VERIFY_D(T, __nv_fp8_e5m2) }
-    else { DISPATCH_VERIFY_D(T, T) }
+    if (cache_dtype == CB_F8E5M2) launch_paged<T, __nv_fp8_e5m2>(a, D);
+    else launch_paged<T, T>(a, D);
   });
-#undef DISPATCH_VERIFY_D
-#undef LAUNCH_VERIFY
-  return CB_LAUNCH_CHECK();
-}
-
-int cb_gather_cos_sin(const float* cos_c, const float* sin_c, const int* pos, float* cos_o, float* sin_o, int tokens,
-                      int half, cudaStream_t s) {
-  if (tokens == 0) return 0;
-  gather_cos_sin_kernel<<<tokens, 128, 0, s>>>(cos_c, sin_c, pos, cos_o, sin_o, tokens, half);
   return CB_LAUNCH_CHECK();
 }
 

@@ -8,8 +8,8 @@ module is the only one that interprets those bytes: the runtime, engine and draf
 from __future__ import annotations
 
 import ctypes
+import functools
 import math
-import os
 from typing import Optional, Tuple
 
 import torch
@@ -81,14 +81,38 @@ def gather_paged_kv(cache: torch.Tensor, block_table: torch.Tensor, length: int,
     return _decode(cache[block_table[:nblk].long()].reshape(-1, cache.shape[2], cache.shape[3])[:length], dtype)
 
 
-def _decode_workspace(q: torch.Tensor, n: int, heads: int, splits: int, head_dim: int):
-    """Persistent split-KV buffers (`inference.flash_decoding_utils.FDIntermTensors`) when the engine set them up."""
+@functools.lru_cache(maxsize=None)
+def sm_count(device_index: int) -> int:
+    """Streaming multiprocessors of CUDA device `device_index`."""
+    return torch.cuda.get_device_properties(device_index).multi_processor_count
+
+
+def decode_splits(num_seqs: int, kv_heads: int, max_len: int, num_sms: int) -> Tuple[int, int]:
+    """Split-KV partition of a paged-attention call over `num_seqs` sequences whose block tables span `max_len`
+    positions: (splits, part_len).  A CTA serves up to 8 kv heads of one sequence and split; the splits aim at two
+    waves of CTAs on `num_sms` SMs, with partitions of at least 64 tokens rounded up to a multiple of 32.  The kernel's
+    partials take [rows, Hq, splits, D] and [rows, Hq, splits, 2] fp32, rows = num_seqs * q_len."""
+    ctas_per_split = num_seqs * ((kv_heads + 7) // 8)
+    splits = (2 * num_sms + ctas_per_split - 1) // ctas_per_split
+    splits = max(1, min(splits, (max_len + 63) // 64))
+    part = (max_len + splits - 1) // splits
+    part = (part + 31) // 32 * 32
+    return max(1, (max_len + part - 1) // part), part
+
+
+def _split_kv_workspace(q: torch.Tensor, rows: int, heads: int, splits: int, head_dim: int):
+    """The split-KV partials (o_part, ml_part) of one call: views of the engine's persistent buffers
+    (`inference.flash_decoding_utils.FDIntermTensors`) when they are set up on q's device and large enough, else
+    fresh tensors."""
     from ..inference.flash_decoding_utils import FDIntermTensors
 
     fd = FDIntermTensors()
-    if not fd.is_initialized or fd.mid_output.device != q.device or fd.mid_output.dtype != torch.float32:
-        return None
-    return fd.views(n, heads, splits, head_dim)
+    if fd.is_initialized and fd.mid_output.device == q.device and fd.mid_output.dtype == torch.float32:
+        ws = fd.views(rows, heads, splits, head_dim)
+        if ws is not None:
+            return ws
+    return (torch.empty(rows, heads, splits, head_dim, dtype=torch.float32, device=q.device),
+            torch.empty(rows, heads, splits, 2, dtype=torch.float32, device=q.device))
 
 
 def paged_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_tables: torch.Tensor,
@@ -101,70 +125,27 @@ def paged_decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torc
     speculative verification of q_len - 1 drafted tokens (one pass over the cache).  `window`: sliding-window attention
     (only the last `window` positions a query sees are visible), handled inside the split-KV kernel (`window_start`).
     An fp8 (uint8) cache is decoded exactly to the query dtype inside the kernel."""
-    if q_len != 1:
-        return _paged_verify_attention(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window, q_len)
-    n, Hq, D = q.shape
-    nb, bs, Hkv, _ = k_cache.shape
-    scale = scale if scale is not None else 1.0 / math.sqrt(D)
-    if (use_native(q) and q.dtype in (torch.float16, torch.bfloat16) and k_cache.dtype in (q.dtype, FP8_CACHE_DTYPE)
-            and D in (64, 128, 256) and Hq // Hkv <= 8):
-        lib = _get_lib()
-        max_len = block_tables.shape[1] * bs
-        part = ctypes.c_int(0)
-        splits = lib.cb_decode_num_splits(n, Hkv, max_len, ctypes.byref(part))
-        out = torch.empty_like(q)
-        ws = _decode_workspace(q, n, Hq, splits, D)
-        if ws is not None:
-            o_part, ml_part = ws
-        else:
-            o_part = torch.empty(n, Hq, splits, D, dtype=torch.float32, device=q.device)
-            ml_part = torch.empty(n, Hq, splits, 2, dtype=torch.float32, device=q.device)
-        qc = q if q.stride(2) == 1 and q.stride(1) == D else q.contiguous()
-        loader.check(lib.cb_paged_decode_attention(
-            loader.ptr(qc), loader.ptr(k_cache), loader.ptr(v_cache), loader.ptr(block_tables), loader.ptr(seq_lens),
-            loader.ptr(out), loader.ptr(o_part), loader.ptr(ml_part), n, Hq, Hkv, D, bs, block_tables.shape[1], splits,
-            part.value, ctypes.c_float(scale), loader.ptr(alibi_slopes), ctypes.c_int64(qc.stride(0)),
-            ctypes.c_int64(out.stride(0)), code(q.dtype), _cache_code(k_cache), int(window or 0), loader.stream_ptr()),
-            "paged_decode_attention")
-        loader.launch_counter.add("paged_decode_attention", 2)
-        return out
-    return paged_decode_attention_ref(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window)
-
-
-def _paged_verify_attention(q, k_cache, v_cache, block_tables, seq_lens, scale, alibi_slopes, window, q_len):
-    """`paged_decode_attention` with q_len query tokens per sequence: one tensor-core pass where the kernel covers the
-    shape, one decode call per query position where only the CUDA-core kernel does (head_dim 256,
-    CB200_DECODE=simt), the reference elsewhere."""
     rows, Hq, D = q.shape
     nb, bs, Hkv, _ = k_cache.shape
     assert q_len >= 1 and rows % q_len == 0, (rows, q_len)
     n = rows // q_len
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     native = (use_native(q) and q.dtype in (torch.float16, torch.bfloat16)
-              and k_cache.dtype in (q.dtype, FP8_CACHE_DTYPE) and Hq // Hkv <= 8)
-    simt = os.environ.get("CB200_DECODE", "").startswith("s")
-    if native and D in (64, 128) and q_len <= 16 and not simt:
-        lib = _get_lib()
-        part = ctypes.c_int(0)
-        splits = lib.cb_decode_num_splits(n, Hkv, block_tables.shape[1] * bs, ctypes.byref(part))
+              and k_cache.dtype in (q.dtype, FP8_CACHE_DTYPE) and D in (64, 128, 256) and Hq // Hkv <= 8)
+    if native and q_len <= (1 if D == 256 else 16):
+        splits, part = decode_splits(n, Hkv, block_tables.shape[1] * bs, sm_count(q.device.index))
         out = torch.empty_like(q)
-        ws = _decode_workspace(q, rows, Hq, splits, D)
-        if ws is not None:
-            o_part, ml_part = ws
-        else:
-            o_part = torch.empty(rows, Hq, splits, D, dtype=torch.float32, device=q.device)
-            ml_part = torch.empty(rows, Hq, splits, 2, dtype=torch.float32, device=q.device)
+        o_part, ml_part = _split_kv_workspace(q, rows, Hq, splits, D)
         qc = q if q.stride(2) == 1 and q.stride(1) == D else q.contiguous()
-        loader.check(lib.cb_paged_verify_attention(
+        loader.check(_get_lib().cb_paged_decode_attention(
             loader.ptr(qc), loader.ptr(k_cache), loader.ptr(v_cache), loader.ptr(block_tables), loader.ptr(seq_lens),
             loader.ptr(out), loader.ptr(o_part), loader.ptr(ml_part), n, q_len, Hq, Hkv, D, bs, block_tables.shape[1],
-            splits, part.value, ctypes.c_float(scale), loader.ptr(alibi_slopes), ctypes.c_int64(qc.stride(0)),
-            ctypes.c_int64(out.stride(0)), code(q.dtype), _cache_code(k_cache), int(window or 0),
-            loader.stream_ptr()),
+            splits, part, ctypes.c_float(scale), loader.ptr(alibi_slopes), ctypes.c_int64(qc.stride(0)),
+            ctypes.c_int64(out.stride(0)), code(q.dtype), _cache_code(k_cache), int(window or 0), loader.stream_ptr()),
             "paged_decode_attention")
         loader.launch_counter.add("paged_decode_attention", 2)
         return out
-    if native and D in (64, 128, 256):
+    if native:          # q_len > 1 beyond the one-pass kernel (head_dim 256, or q_len > 16): one decode call per query
         qs = q.view(n, q_len, Hq, D)
         outs = [paged_decode_attention(qs[:, j], k_cache, v_cache, block_tables, seq_lens - (q_len - 1 - j), scale,
                                        alibi_slopes, window) for j in range(q_len)]

@@ -2,7 +2,6 @@
 block 16).  Decode is bound by HBM bandwidth, so the figure of merit is bytes read per second: the cache K+V at its
 element size plus q, the output and the split-KV partials (written and read back).  The bf16 cache holds the decoded
 fp8 cache, so both runs compute the same values and their outputs must be bitwise equal."""
-import ctypes
 import json
 import subprocess
 
@@ -47,7 +46,7 @@ def main():
     assert torch.cuda.is_available(), "bench_paged_decode.py measures the GPU kernels and needs a GPU"
     print("GPU " + json.dumps(gpu_info()), flush=True)
     dev = torch.device("cuda")
-    lib = iops._get_lib()
+    sms = iops.sm_count(torch.cuda.current_device())
     for B in (1, 16, 64):
         for L in (1024, 4096, 16384):
             torch.manual_seed(0)
@@ -59,8 +58,7 @@ def main():
             kc8, vc8 = kc8.view(torch.uint8), vc8.view(torch.uint8)
             lens = torch.full((B,), L, device=dev, dtype=torch.int32)
             q = torch.randn(B, HQ, D, device=dev, dtype=torch.bfloat16)
-            part = ctypes.c_int(0)
-            splits = lib.cb_decode_num_splits(B, HKV, L, ctypes.byref(part))
+            splits, _ = iops.decode_splits(B, HKV, L, sms)
             other = 2 * B * HQ * D * 2 + 2 * B * HQ * splits * (D + 2) * 4     # q + out, partials written and read
             same = torch.equal(iops.paged_decode_attention(q, kc8, vc8, tables, lens),
                                iops.paged_decode_attention(q, kc16, vc16, tables, lens))

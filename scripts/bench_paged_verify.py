@@ -4,7 +4,6 @@ each with its own sequence lengths).  Both are timed at every shape and must giv
 counted as in bench_paged_decode.py - the cache K+V once at its element size, plus q, the output and the split-KV
 partials of all n query rows - so the loop's rate is the useful rate, not the bytes it actually moves (n times the
 cache)."""
-import ctypes
 import json
 
 import torch
@@ -24,7 +23,7 @@ def main():
     assert torch.cuda.is_available(), "bench_paged_verify.py measures the GPU kernels and needs a GPU"
     print("GPU " + json.dumps(gpu_info()), flush=True)
     dev = torch.device("cuda")
-    lib = iops._get_lib()
+    sms = iops.sm_count(torch.cuda.current_device())
     for B in (1, 16, 64):
         for L in (1024, 4096, 16384):
             torch.manual_seed(0)
@@ -35,8 +34,7 @@ def main():
             caches = {"bf16": (kc8.to(torch.bfloat16), vc8.to(torch.bfloat16)),
                       "fp8": (kc8.view(torch.uint8), vc8.view(torch.uint8))}
             lens = torch.full((B,), L, device=dev, dtype=torch.int32)
-            part = ctypes.c_int(0)
-            splits = lib.cb_decode_num_splits(B, HKV, L, ctypes.byref(part))
+            splits, _ = iops.decode_splits(B, HKV, L, sms)
             for name, (kc, vc) in caches.items():
                 for q_len in (1, 2, 4, 6):
                     q = torch.randn(B * q_len, HQ, D, device=dev, dtype=torch.bfloat16)

@@ -40,6 +40,24 @@ def test_reference_q_len_equals_per_row_loop(fp8, alibi, window, q_len):
     assert torch.equal(got, _per_row_reference(q, kc, vc, tables, lens, q_len, **kw))
 
 
+# (num_seqs, kv_heads, max_len) -> (splits, part_len) on 132 SMs (H100 SXM), as computed by the native
+# `cb_decode_num_splits` that `decode_splits` replaces.  A verify pass uses the decode step's splits, which keeps each
+# of its rows bitwise equal to the single-query result.
+_SPLITS_132_SMS = {
+    (1, 8, 1): (1, 32), (1, 8, 31): (1, 32), (1, 8, 100): (2, 64), (1, 8, 1000): (16, 64), (1, 8, 4096): (64, 64),
+    (1, 8, 4097): (65, 64), (1, 8, 16384): (256, 64), (1, 16, 16384): (128, 128),
+    (16, 8, 1): (1, 32), (16, 8, 31): (1, 32), (16, 8, 100): (2, 64), (16, 8, 1000): (16, 64),
+    (16, 8, 4096): (16, 256), (16, 8, 4097): (17, 256), (16, 8, 16384): (17, 992), (16, 16, 4096): (9, 480),
+    (64, 8, 1): (1, 32), (64, 8, 31): (1, 32), (64, 8, 100): (2, 64), (64, 8, 1000): (5, 224),
+    (64, 8, 4096): (5, 832), (64, 8, 4097): (5, 832), (64, 8, 16384): (5, 3296), (64, 16, 1000): (3, 352),
+}
+
+
+@pytest.mark.parametrize("shape", sorted(_SPLITS_132_SMS))
+def test_decode_splits_pinned_table(shape):
+    assert iops.decode_splits(*shape, 132) == _SPLITS_132_SMS[shape]
+
+
 def _spec_vs_plain(model, cfg_kw, prompts, n_new, n_spec):
     torch.manual_seed(1)
     drafter = build_model(get_config("llama-tiny", num_hidden_layers=1)).float().eval()

@@ -99,38 +99,39 @@ def test_paged_decode_fp8_long_context_split_kv():
     _check_decode(torch.randn(2, 32, 128, device=dev, dtype=torch.bfloat16), kc, vc, tables, lens)
 
 
+@pytest.mark.parametrize("D", [128, 256])          # tensor-core and CUDA-core kernels
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-def test_paged_decode_fp8_alibi(dtype):
+def test_paged_decode_fp8_alibi(dtype, D):
     dev = torch.device("cuda")
     torch.manual_seed(2)
-    kc, vc, tables = _mk_fp8_cache(3, 256, 16, 8, 128, dev)
+    kc, vc, tables = _mk_fp8_cache(3, 256, 16, 8, D, dev)
     lens = torch.tensor([5, 100, 256], device=dev, dtype=torch.int32)
     slopes = torch.tensor([2 ** (-(i + 1)) for i in range(8)], device=dev, dtype=torch.float32)
-    _check_decode(torch.randn(3, 8, 128, device=dev, dtype=dtype), kc, vc, tables, lens, alibi_slopes=slopes)
+    _check_decode(torch.randn(3, 8, D, device=dev, dtype=dtype), kc, vc, tables, lens, alibi_slopes=slopes)
 
 
+@pytest.mark.parametrize("D", [128, 256])          # tensor-core and CUDA-core kernels
 @pytest.mark.parametrize("window", [1, 16, 100, 4096])
 @pytest.mark.parametrize("alibi", [False, True])
-def test_paged_decode_fp8_sliding_window(window, alibi):
+def test_paged_decode_fp8_sliding_window(window, alibi, D):
     dev = torch.device("cuda")
     torch.manual_seed(3)
-    kc, vc, tables = _mk_fp8_cache(5, 3000, 16, 4, 128, dev)
+    kc, vc, tables = _mk_fp8_cache(5, 3000, 16, 4, D, dev)
     lens = torch.tensor([1, 15, 100, 1025, 3000], device=dev, dtype=torch.int32)
     slopes = torch.tensor([2 ** (-(i + 1) / 2) for i in range(16)], device=dev, dtype=torch.float32) if alibi else None
-    _check_decode(torch.randn(5, 16, 128, device=dev, dtype=torch.bfloat16), kc, vc, tables, lens,
+    _check_decode(torch.randn(5, 16, D, device=dev, dtype=torch.bfloat16), kc, vc, tables, lens,
                   alibi_slopes=slopes, window=window)
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("group", [1, 4, 8])
-def test_paged_decode_fp8_simt_kernel(monkeypatch, dtype, group):
-    """CB200_DECODE=simt selects the CUDA-core kernel at head_dim 128 (the one head_dim 256 always uses)."""
-    monkeypatch.setenv("CB200_DECODE", "simt")
+def test_paged_decode_fp8_simt_kernel(dtype, group):
+    """The CUDA-core kernel (head_dim 256) around block and partition boundaries."""
     dev = torch.device("cuda")
     torch.manual_seed(4)
-    kc, vc, tables = _mk_fp8_cache(7, 700, 16, 2, 128, dev)
+    kc, vc, tables = _mk_fp8_cache(7, 700, 16, 2, 256, dev)
     lens = torch.tensor([1, 15, 16, 17, 300, 699, 700], device=dev, dtype=torch.int32)
-    _check_decode(torch.randn(7, 2 * group, 128, device=dev, dtype=dtype), kc, vc, tables, lens)
+    _check_decode(torch.randn(7, 2 * group, 256, device=dev, dtype=dtype), kc, vc, tables, lens)
 
 
 def test_engine_fp8_cache_native_graphs_and_rounded_write_oracle(monkeypatch):

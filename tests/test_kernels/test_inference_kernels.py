@@ -81,15 +81,16 @@ def test_paged_decode_grid(bsz, bs, max_blocks, group, D, same_len):
     torch.testing.assert_close(out.float(), ref, atol=2e-2, rtol=2e-2)
 
 
+@pytest.mark.parametrize("D", [128, 256])          # tensor-core and CUDA-core kernels
 @pytest.mark.parametrize("window", [1, 16, 100, 4096])
 @pytest.mark.parametrize("alibi", [False, True])
-def test_paged_decode_sliding_window(window, alibi):
+def test_paged_decode_sliding_window(window, alibi, D):
     """`window_start` inside the split-KV kernel: only the last `window` cached tokens are visible."""
     dev = torch.device("cuda")
     torch.manual_seed(3)
-    kc, vc, tables = _mk_cache(5, 3000, 16, 4, 128, torch.bfloat16, dev)
+    kc, vc, tables = _mk_cache(5, 3000, 16, 4, D, torch.bfloat16, dev)
     lens = torch.tensor([1, 15, 100, 1025, 3000], device=dev, dtype=torch.int32)
-    q = torch.randn(5, 16, 128, device=dev, dtype=torch.bfloat16)
+    q = torch.randn(5, 16, D, device=dev, dtype=torch.bfloat16)
     slopes = torch.tensor([2 ** (-(i + 1) / 2) for i in range(16)], device=dev, dtype=torch.float32) if alibi else None
     out = iops.paged_decode_attention(q, kc, vc, tables, lens, alibi_slopes=slopes, window=window)
     ref = iops.paged_decode_attention_ref(q.float(), kc.float(), vc.float(), tables, lens, alibi_slopes=slopes,

@@ -9,8 +9,10 @@ import torch
 
 from colossalai_b200.kernel import loader
 from colossalai_b200.ops import inference as iops
+from colossalai_b200.ops._dtypes import code
 
 pytestmark = pytest.mark.gpu
+CUDA_ERROR_INVALID_VALUE = 1
 
 
 def _per_position(q, kc, vc, tables, lens, q_len, decode=None, **kw):
@@ -122,35 +124,45 @@ def test_paged_verify_sliding_window(window, alibi, fp8):
 
 
 @pytest.mark.parametrize("fp8", [False, True])
-def test_paged_verify_long_context_split_kv(fp8):
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_paged_verify_long_context_split_kv(dtype, fp8):
     """8192-token split-KV; some rows of a sequence end below the start of a split its last row reaches."""
     dev = torch.device("cuda")
     torch.manual_seed(1)
-    part = ctypes.c_int(0)
-    iops._get_lib().cb_decode_num_splits(3, 8, 8192, ctypes.byref(part))
-    P = part.value
+    _, P = iops.decode_splits(3, 8, 8192, iops.sm_count(torch.cuda.current_device()))
     k, v, tables = _caches(3, 8192, 16, 8, 128, dev)
     lens = torch.tensor([8192, 2 * P + 1, 3 * P + 2], device=dev, dtype=torch.int32)
-    q = torch.randn(3 * 6, 32, 128, device=dev, dtype=torch.bfloat16)
-    _check(q, _as_cache(k, torch.bfloat16, fp8), _as_cache(v, torch.bfloat16, fp8), tables, lens, 6)
+    q = torch.randn(3 * 6, 32, 128, device=dev, dtype=dtype)
+    _check(q, _as_cache(k, dtype, fp8), _as_cache(v, dtype, fp8), tables, lens, 6)
 
 
 @pytest.mark.parametrize("fp8", [False, True])
-@pytest.mark.parametrize("D,simt", [(256, False), (128, True)])
-def test_paged_verify_cuda_core_shapes_run_the_loop(monkeypatch, D, simt, fp8):
-    """Shapes only the CUDA-core kernel serves run one decode call per query position: exactly the loop's output."""
-    if simt:
-        monkeypatch.setenv("CB200_DECODE", "simt")
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_paged_verify_cuda_core_shapes_run_the_loop(dtype, fp8):
+    """Head_dim 256, which only the CUDA-core kernel serves, runs one decode call per query position: exactly the
+    loop's output.  The native launcher itself refuses q_len > 1 there and launches nothing."""
+    D = 256
     dev = torch.device("cuda")
     torch.manual_seed(4)
     k, v, tables = _caches(4, 300, 16, 2, D, dev)
-    kc, vc = _as_cache(k, torch.bfloat16, fp8), _as_cache(v, torch.bfloat16, fp8)
+    kc, vc = _as_cache(k, dtype, fp8), _as_cache(v, dtype, fp8)
     lens = torch.tensor([3, 17, 200, 300], device=dev, dtype=torch.int32)
-    q = torch.randn(4 * 3, 8, D, device=dev, dtype=torch.bfloat16)
+    q = torch.randn(4 * 3, 8, D, device=dev, dtype=dtype)
     loader.launch_counter.reset()
     out = iops.paged_decode_attention(q, kc, vc, tables, lens, q_len=3)
     assert loader.launch_counter.by_name["paged_decode_attention"] == 2 * 3
     assert torch.equal(out, _per_position(q, kc, vc, tables, lens, 3))
+
+    q2, out2 = q[: 4 * 2].contiguous(), torch.zeros(4 * 2, 8, D, device=dev, dtype=dtype)
+    o_part, ml_part = torch.empty(4 * 2, 8, 1, D, device=dev), torch.empty(4 * 2, 8, 1, 2, device=dev)
+    err = iops._get_lib().cb_paged_decode_attention(
+        loader.ptr(q2), loader.ptr(kc), loader.ptr(vc), loader.ptr(tables), loader.ptr(lens), loader.ptr(out2),
+        loader.ptr(o_part), loader.ptr(ml_part), 4, 2, 8, 2, D, 16, tables.shape[1], 1, 320, ctypes.c_float(D ** -0.5),
+        loader.ptr(None), ctypes.c_int64(q2.stride(0)), ctypes.c_int64(out2.stride(0)), code(dtype),
+        iops._cache_code(kc), 0, loader.stream_ptr())
+    torch.cuda.synchronize()
+    assert err == CUDA_ERROR_INVALID_VALUE
+    assert not out2.any()
 
 
 def test_paged_verify_is_one_native_call():
