@@ -10,14 +10,18 @@
 
 CB_DEVICE float silu_f(float x) { return x / (1.f + __expf(-x)); }
 CB_DEVICE float sigmoid_f(float x) { return 1.f / (1.f + __expf(-x)); }
+// tanh-approximated GELU, 0.5 x (1 + tanh u) with u = k (x + 0.044715 x^3), evaluated as x * sigmoid(2u).  The two
+// are equal, but `tanhf` compiles to the tanh.approx unit under --use_fast_math (relative error 2^-11), and
+// 1 + tanh u cancels for negative x; the sigmoid form has neither problem.
 CB_DEVICE float gelu_tanh_f(float x) {
   const float k = 0.7978845608028654f;
-  return 0.5f * x * (1.f + tanhf(k * (x + 0.044715f * x * x * x)));
+  return x * sigmoid_f(2.f * k * (x + 0.044715f * x * x * x));
 }
+// d/dx = s + x * 2 s (1 - s) * u'  with s = sigmoid(2u)  (0.5 (1 + tanh u) = s, 1 - tanh^2 u = 4 s (1 - s))
 CB_DEVICE float gelu_tanh_grad_f(float x) {
   const float k = 0.7978845608028654f;
-  const float t = tanhf(k * (x + 0.044715f * x * x * x));
-  return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * k * (1.f + 3.f * 0.044715f * x * x);
+  const float s = sigmoid_f(2.f * k * (x + 0.044715f * x * x * x));
+  return s + 2.f * x * s * (1.f - s) * k * (1.f + 3.f * 0.044715f * x * x);
 }
 CB_DEVICE float gelu_erf_f(float x) { return 0.5f * x * (1.f + erff(x * 0.7071067811865476f)); }
 CB_DEVICE float gelu_erf_grad_f(float x) {

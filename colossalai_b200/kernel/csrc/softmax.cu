@@ -1,7 +1,7 @@
 // Scaled masked softmax and scaled upper-triangular (causal) masked softmax, forward + backward.
 // Behavioural parity: reference extensions/csrc/kernel/cuda/scaled_masked_softmax_kernel.cu (fwd :35, bwd :158) and
 // scaled_upper_triang_masked_softmax_kernel.cu (fwd :35, bwd :157): y = softmax(scale * x masked_fill(mask, -10000)).
-// Design here: one warp per row for sk <= 4096 (row lives in registers, two shuffles reductions), one CTA per row
+// Design here: one warp per row for sk <= 1024 (row lives in registers, two shuffles reductions), one CTA per row
 // beyond that (no 2048-key limit as in the reference); fp32 math, 16-bit or fp32 I/O.
 #include "common.cuh"
 

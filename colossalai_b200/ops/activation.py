@@ -12,6 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from ..kernel import loader
+from ._align import aligned
 from ._dispatch import use_native
 from ._dtypes import code
 
@@ -45,7 +46,7 @@ class _GLUFn(torch.autograd.Function):
         lib = _get_lib()
         shape = gate_up.shape
         I = shape[-1] // 2
-        gu = gate_up.contiguous().view(-1, 2 * I)
+        gu = aligned(gate_up.contiguous().view(-1, 2 * I))
         out = torch.empty(gu.shape[0], I, dtype=gu.dtype, device=gu.device)
         loader.check(lib.cb_glu_fwd_bounded(loader.ptr(gu), loader.ptr(out), ctypes.c_int64(gu.shape[0]), I, act,
                                             code(gu.dtype), loader.ptr(valid_rows), loader.stream_ptr()), "glu_fwd")
@@ -60,7 +61,7 @@ class _GLUFn(torch.autograd.Function):
         gu, vr = ctx.saved_tensors
         vr = vr if vr.numel() else None
         I = gu.shape[1] // 2
-        d = dout.contiguous().view(-1, I)
+        d = aligned(dout.contiguous().view(-1, I))
         dgu = torch.empty_like(gu)
         loader.check(lib.cb_glu_bwd_bounded(loader.ptr(d), loader.ptr(gu), loader.ptr(dgu), ctypes.c_int64(gu.shape[0]),
                                             I, ctx.act, code(gu.dtype), loader.ptr(vr), loader.stream_ptr()), "glu_bwd")
@@ -92,7 +93,8 @@ class _BiasActFn(torch.autograd.Function):
         lib = _get_lib()
         shape = x.shape
         H = shape[-1]
-        x2 = x.contiguous().view(-1, H)
+        x2 = aligned(x.contiguous().view(-1, H))
+        bias = aligned(bias)
         y = torch.empty_like(x2)
         loader.check(lib.cb_bias_act_fwd(loader.ptr(x2), loader.ptr(bias), loader.ptr(y), ctypes.c_int64(x2.shape[0]),
                                          H, act, code(x.dtype), loader.stream_ptr()), "bias_act_fwd")
@@ -106,7 +108,7 @@ class _BiasActFn(torch.autograd.Function):
         lib = _get_lib()
         x2, bias = ctx.saved_tensors
         H = x2.shape[1]
-        d = dy.contiguous().view(-1, H)
+        d = aligned(dy.contiguous().view(-1, H))
         dx = torch.empty_like(x2)
         loader.check(lib.cb_bias_act_bwd(loader.ptr(d), loader.ptr(x2), loader.ptr(bias), loader.ptr(dx),
                                          ctypes.c_int64(x2.shape[0]), H, ctx.act, code(x2.dtype),

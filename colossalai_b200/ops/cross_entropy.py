@@ -11,6 +11,7 @@ from typing import Optional
 import torch
 
 from ..kernel import loader
+from ._align import aligned
 from ._dispatch import use_native
 from ._dtypes import code
 
@@ -34,6 +35,7 @@ def row_max(logits: torch.Tensor, valid_cols: Optional[int] = None) -> torch.Ten
     Vv = logits.shape[-1] if valid_cols is None else valid_cols
     if _ok(logits):
         lib = _get_lib()
+        logits = aligned(logits)   # rows are read as 16-byte vectors
         T, V = logits.shape
         out = torch.empty(T, dtype=torch.float32, device=logits.device)
         loader.check(lib.cb_ce_row_max(loader.ptr(logits), loader.ptr(out), T, V, Vv, code(logits.dtype),
@@ -50,9 +52,10 @@ def sumexp_and_target(logits: torch.Tensor, target: torch.Tensor, gmax: torch.Te
     Vv = V if valid_cols is None else valid_cols
     if _ok(logits):
         lib = _get_lib()
+        logits = aligned(logits)
         out = torch.empty(2, T, dtype=torch.float32, device=logits.device)
-        tgt = target if target.dtype == torch.int64 else target.long()
-        loader.check(lib.cb_ce_sumexp_target(loader.ptr(logits), loader.ptr(tgt.contiguous()), loader.ptr(gmax),
+        tgt = (target if target.dtype == torch.int64 else target.long()).contiguous()
+        loader.check(lib.cb_ce_sumexp_target(loader.ptr(logits), loader.ptr(tgt), loader.ptr(gmax),
                                              loader.ptr(out), T, V, Vv, ctypes.c_int64(vocab_start),
                                              ctypes.c_int64(ignore_index), code(logits.dtype),
                                              loader.stream_ptr()), "ce_sumexp_target")
@@ -76,13 +79,15 @@ def softmax_grad(logits: torch.Tensor, target: torch.Tensor, gmax: torch.Tensor,
     T, V = logits.shape
     Vv = V if valid_cols is None else valid_cols
     if row_scale is None:
-        row_scale = scale.reshape(1).expand(T).contiguous().float()
+        row_scale = scale.reshape(1).expand(T)
+    row_scale = row_scale.float().contiguous()
     if _ok(logits):
         lib = _get_lib()
+        logits = aligned(logits)
         out = torch.empty_like(logits)
-        tgt = target if target.dtype == torch.int64 else target.long()
-        loader.check(lib.cb_ce_softmax_grad(loader.ptr(logits), loader.ptr(tgt.contiguous()), loader.ptr(gmax),
-                                            loader.ptr(sumexp), loader.ptr(row_scale.contiguous()), loader.ptr(out),
+        tgt = (target if target.dtype == torch.int64 else target.long()).contiguous()
+        loader.check(lib.cb_ce_softmax_grad(loader.ptr(logits), loader.ptr(tgt), loader.ptr(gmax),
+                                            loader.ptr(sumexp), loader.ptr(row_scale), loader.ptr(out),
                                             T, V, Vv, ctypes.c_int64(vocab_start), ctypes.c_int64(ignore_index),
                                             code(logits.dtype), loader.stream_ptr()), "ce_softmax_grad")
         loader.launch_counter.add("ce_softmax_grad")

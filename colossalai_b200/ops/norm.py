@@ -12,6 +12,7 @@ from typing import Optional, Tuple
 import torch
 
 from ..kernel import loader
+from ._align import aligned
 from ._dispatch import use_native
 from ._dtypes import code
 
@@ -59,13 +60,14 @@ class _RMSNormFn(torch.autograd.Function):
         lib = _get_lib()
         shape = x.shape
         H = shape[-1]
-        x2 = x.contiguous().view(-1, H)
+        x2 = aligned(x.contiguous().view(-1, H))
+        weight = aligned(weight)
         rows = x2.shape[0]
         y = torch.empty_like(x2)
         rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
         has_res = residual is not None
         if has_res:
-            r2 = residual.contiguous().view(-1, H)
+            r2 = aligned(residual.contiguous().view(-1, H))
             h = torch.empty_like(x2)
         else:
             r2, h = None, x2
@@ -85,8 +87,8 @@ class _RMSNormFn(torch.autograd.Function):
         lib = _get_lib()
         h, weight, rstd = ctx.saved_tensors
         rows, H = h.shape
-        dy2 = dy.contiguous().view(-1, H)
-        dres = dh.contiguous().view(-1, H) if (ctx.has_res and dh is not None) else None
+        dy2 = aligned(dy.contiguous().view(-1, H))
+        dres = aligned(dh.contiguous().view(-1, H)) if (ctx.has_res and dh is not None) else None
         dx = torch.empty_like(h)
         grid = lib.cb_norm_bwd_grid(rows)
         partial = torch.empty(grid, H, dtype=torch.float32, device=h.device)
@@ -113,7 +115,8 @@ class _LayerNormFn(torch.autograd.Function):
         lib = _get_lib()
         shape = x.shape
         H = shape[-1]
-        x2 = x.contiguous().view(-1, H)
+        x2 = aligned(x.contiguous().view(-1, H))
+        weight, bias = aligned(weight), aligned(bias)
         rows = x2.shape[0]
         y = torch.empty_like(x2)
         mean = torch.empty(rows, dtype=torch.float32, device=x.device)
@@ -132,7 +135,7 @@ class _LayerNormFn(torch.autograd.Function):
         lib = _get_lib()
         x2, weight, mean, rstd = ctx.saved_tensors
         rows, H = x2.shape
-        dy2 = dy.contiguous().view(-1, H)
+        dy2 = aligned(dy.contiguous().view(-1, H))
         dx = torch.empty_like(x2)
         grid = lib.cb_norm_bwd_grid(rows)
         pw = torch.empty(grid, H, dtype=torch.float32, device=x2.device)

@@ -11,6 +11,7 @@ from typing import Optional, Tuple
 import torch
 
 from ..kernel import loader
+from ._align import VEC_BYTES, rows_aligned
 from ._dispatch import use_native
 from ._dtypes import code
 
@@ -65,6 +66,15 @@ def rope_ref(x: torch.Tensor, positions: Optional[torch.Tensor], cos: torch.Tens
 
 def _native_rope_(qkv2d: torch.Tensor, positions, cos, sin, n_rot_heads: int, D: int, rot_dim: int, sign: float,
                   interleaved: bool) -> None:
+    if not rows_aligned(qkv2d):
+        # the kernel rotates 16-byte vectors of each row: rotate an aligned copy with padded rows, then copy back
+        vec = VEC_BYTES // qkv2d.element_size()
+        T, W = qkv2d.shape
+        tmp = torch.empty(T, -(-W // vec) * vec, dtype=qkv2d.dtype, device=qkv2d.device)[:, :W]
+        tmp.copy_(qkv2d)
+        _native_rope_(tmp, positions, cos, sin, n_rot_heads, D, rot_dim, sign, interleaved)
+        qkv2d.copy_(tmp)
+        return
     lib = _get_lib()
     loader.check(lib.cb_rope(loader.ptr(qkv2d), loader.ptr(positions), loader.ptr(cos), loader.ptr(sin),
                              ctypes.c_int64(qkv2d.shape[0]), ctypes.c_int64(qkv2d.stride(0)), n_rot_heads, D,

@@ -33,8 +33,11 @@ def scaled_causal_softmax_ref(x: torch.Tensor, scale: float) -> torch.Tensor:
     sq, sk = x.shape[-2:]
     s = x.float() * scale
     keep = torch.ones(sq, sk, dtype=torch.bool, device=x.device).tril(diagonal=sk - sq)
-    s = s.masked_fill(~keep, float("-inf"))
-    return torch.softmax(s, dim=-1).to(x.dtype)
+    # with sq > sk the first sq - sk queries see no key: the kernel writes zeros there (softmax would give NaN),
+    # and those rows are kept finite before the softmax so that its backward stays finite too
+    empty = ~keep.any(-1, keepdim=True)
+    s = s.masked_fill(~keep, float("-inf")).masked_fill(empty, 0.0)
+    return torch.softmax(s, dim=-1).masked_fill(empty, 0.0).to(x.dtype)
 
 
 class _ScaledMaskedSoftmax(torch.autograd.Function):

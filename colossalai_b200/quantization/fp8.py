@@ -18,6 +18,7 @@ import torch.distributed as dist
 import torch.nn.functional as F
 
 from ..kernel import loader
+from ..ops._align import aligned
 from ..ops._dispatch import use_native
 from ..ops._dtypes import code
 
@@ -76,7 +77,7 @@ def cast_to_fp8(inp: torch.Tensor, fp8_format: str = "e4m3", per_channel_scale: 
     if use_native(inp) and inp.is_contiguous():
         lib = _get_lib()
         q = out.view(torch.uint8) if out is not None else torch.empty(inp.shape, dtype=torch.uint8, device=inp.device)
-        if per_channel_scale:
+        if per_channel_scale:   # scalar loads and stores: any address
             rows, cols = inp.numel() // inp.shape[-1], inp.shape[-1]
             sinv = torch.empty(rows, dtype=torch.float32, device=inp.device)
             loader.check(lib.cb_fp8_quant_rows(loader.ptr(inp), loader.ptr(q), rows, cols, ctypes.c_int64(cols),
@@ -84,12 +85,17 @@ def cast_to_fp8(inp: torch.Tensor, fp8_format: str = "e4m3", per_channel_scale: 
                                                loader.stream_ptr()), "fp8_quant_rows")
             loader.launch_counter.add("fp8_quant_rows")
             return q.view(fp8_type), sinv.unsqueeze(0)
+        # the per-tensor kernels read 16-byte vectors of `inp` and write 16 / elsize bytes of `q` at a time
+        inp = aligned(inp)
+        q_out, q = q, aligned(q, 16 // inp.element_size())
         buf = torch.empty(2, dtype=torch.float32, device=inp.device)
         loader.check(lib.cb_fp8_quant_tensor(loader.ptr(inp), loader.ptr(q), ctypes.c_int64(inp.numel()),
                                              loader.ptr(buf[0:1]), loader.ptr(buf[1:2]), code(inp.dtype),
                                              _FMT_CODE[fp8_format], loader.stream_ptr()), "fp8_quant_tensor")
         loader.launch_counter.add("fp8_quant_tensor", 2)
-        return q.view(fp8_type), buf[1:2]
+        if q is not q_out:
+            q_out.copy_(q)
+        return q_out.view(fp8_type), buf[1:2]
     if per_channel_scale:
         amax = inp.abs().max(dim=-1).values.float()
         amax = torch.where(amax > 0, amax, torch.ones_like(amax))
@@ -113,6 +119,7 @@ def cast_from_fp8(inp: torch.Tensor, scale_inv: torch.Tensor, ret_type: torch.dt
         return inp.to(ret_type)
     if use_native(inp) and inp.is_contiguous() and ret_type in (torch.float32, torch.float16, torch.bfloat16):
         dst = out if out is not None else torch.empty(inp.shape, dtype=ret_type, device=inp.device)
+        inp = aligned(inp, 4)   # read as 4-byte words; `dst` is written element by element
         sinv = scale_inv.reshape(-1).float().contiguous()
         cols = inp.shape[-1] if per_channel_scale else 0
         fmt = 0 if inp.dtype == torch.float8_e4m3fn else 1
