@@ -335,8 +335,8 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 template <int D>
 int launch_flash_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int batch, int seqlen_q,
                      int seqlen_k, int hq, int hkv, int causal, float scale, int dtype, cudaStream_t stream,
-                     const int* cu_seqlens = nullptr, long long total_tokens = 0, float* o_state = nullptr,
-                     int has_prev = 0, int window = 0, const float* alibi = nullptr) {
+                     const int* cu_seqlens, long long total_tokens, float* o_state, int has_prev, int window,
+                     const float* alibi) {
   using C = FaCfg<D>;
   const bool bf16 = dtype == CB_BF16;
   CUtensorMap tq, tk, tv;
@@ -755,83 +755,75 @@ int launch_flash_bwd(const void* q, const void* k, const void* v, const void* do
   return (int)cudaGetLastError();
 }
 
+// dtype validated by the caller (bf16 or fp16)
+int launch_flash_delta(const void* out, const void* dout, float* delta, long long rows, int head_dim, int dtype,
+                       cudaStream_t stream) {
+  const int wpb = 8;
+  const unsigned blocks = (unsigned)((rows + wpb - 1) / wpb);
+  if (dtype == CB_BF16)
+    flash_bwd_delta_kernel<__nv_bfloat16><<<blocks, wpb * 32, 0, stream>>>(
+        (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta, rows, head_dim);
+  else
+    flash_bwd_delta_kernel<__half><<<blocks, wpb * 32, 0, stream>>>((const __half*)out, (const __half*)dout, delta,
+                                                                    rows, head_dim);
+  return (int)cudaGetLastError();
+}
+
+// the envelope of the wgmma backward kernel, shared by both backward entry points
+bool bwd_args_ok(int hq, int hkv, int head_dim, int dtype) {
+  return hkv > 0 && hq % hkv == 0 && head_dim == 128 && (dtype == CB_BF16 || dtype == CB_F16);
+}
+
 }  // namespace
 
 extern "C" {
 
-// q [batch * seqlen_q, hq, D], k / v [batch * seqlen_k, hkv, D] contiguous token-major; out like q; lse [batch *
-// seqlen_q, hq] fp32 (may be null).  Requirements: D in {64, 128}, causal => seqlen_q == seqlen_k
-// (any lengths: partial tiles are masked), hq % hkv == 0, 16-byte aligned bases.
-int cb_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int batch, int seqlen_q,
-                      int seqlen_k, int hq, int hkv, int head_dim, int causal, float scale, int dtype,
+// The one forward entry point.  q [rows_q, hq, D], k / v [rows_k, hkv, D] contiguous token-major, 16-byte aligned
+// bases; out like q; lse [rows_q, hq] fp32 natural log (may be null except in block mode).  Sequence lengths need not
+// be multiples of the tile: partial tiles are masked (keys) / not stored (queries).  The arguments select the mode:
+//   uniform : cu_seqlens null, `batch` sequences of seqlen_q queries / seqlen_k keys (causal => seqlen_q == seqlen_k);
+//   packed  : cu_seqlens int32[batch + 1] ON THE DEVICE, self attention over `total_tokens` rows (seqlen_q / seqlen_k
+//             ignored).  The host never reads the boundaries: the grid is sized for the worst case and surplus CTAs
+//             exit.  Reference counterpart: `flash_attn_varlen_kvpacked_func` behind
+//             `extensions/pybind/flash_attention/flash_attention_dao_cuda.py:37-96`;
+//   prefill : packed and causal with a sliding window (`window` > 0: query q sees keys (q - window, q]; Mistral) and /
+//             or ALiBi slopes (`alibi` [hq] fp32: score += slope * (key - query); BLOOM, Baichuan-13B);
+//   block   : o_state non-null, uniform only (ring attention, see below): the fp32 online-softmax state (o_state
+//             [rows_q, hq, D], lse) is written instead of `out`, and read first when `has_prev`.
+// Anything outside that envelope returns cudaErrorInvalidValue and launches nothing.
+int cb_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, float* o_state, int has_prev,
+                      const int* cu_seqlens, long long total_tokens, int batch, int seqlen_q, int seqlen_k, int hq,
+                      int hkv, int head_dim, int causal, float scale, int window, const float* alibi, int dtype,
                       cudaStream_t stream) {
-  if (batch <= 0 || seqlen_q <= 0) return 0;
-  if (hq % hkv || (causal && seqlen_q != seqlen_k)) return (int)cudaErrorInvalidValue;
-  // sequence lengths need not be multiples of the tile: partial tiles are masked (keys) / not stored (queries)
-  if (dtype != CB_BF16 && dtype != CB_F16) return (int)cudaErrorInvalidValue;
-  if (head_dim == 128)
-    return launch_flash_fwd<128>(q, k, v, out, lse, batch, seqlen_q, seqlen_k, hq, hkv, causal, scale, dtype, stream);
-  if (head_dim == 64)
-    return launch_flash_fwd<64>(q, k, v, out, lse, batch, seqlen_q, seqlen_k, hq, hkv, causal, scale, dtype, stream);
-  return (int)cudaErrorInvalidValue;
-}
-
-// Packed (variable-length) self attention: q / k / v [total_tokens, heads, D]; cu_seqlens int32[batch + 1] ON THE DEVICE
-// (never read by the host: the grid is sized for the worst case and surplus CTAs exit).  Reference counterpart:
-// `flash_attn_varlen_kvpacked_func` behind `extensions/pybind/flash_attention/flash_attention_dao_cuda.py:37-96`.
-int cb_flash_attn_varlen_fwd(const void* q, const void* k, const void* v, void* out, float* lse, const int* cu_seqlens,
-                             int batch, long long total_tokens, int hq, int hkv, int head_dim, int causal, float scale,
-                             int dtype, cudaStream_t stream) {
-  if (batch <= 0 || total_tokens <= 0) return 0;
-  if (hq % hkv || (dtype != CB_BF16 && dtype != CB_F16) || cu_seqlens == nullptr) return (int)cudaErrorInvalidValue;
-  if (head_dim == 128)
-    return launch_flash_fwd<128>(q, k, v, out, lse, batch, 0, 0, hq, hkv, causal, scale, dtype, stream, cu_seqlens, total_tokens);
-  if (head_dim == 64)
-    return launch_flash_fwd<64>(q, k, v, out, lse, batch, 0, 0, hq, hkv, causal, scale, dtype, stream, cu_seqlens, total_tokens);
-  return (int)cudaErrorInvalidValue;
-}
-
-// Packed causal forward for inference prefill with a sliding window (Mistral: query q sees keys (q - window, q]) and /
-// or ALiBi slopes ([hq] fp32: score += slope * (key - query); BLOOM, Baichuan-13B).  Forward only.
-int cb_flash_attn_varlen_fwd_ex(const void* q, const void* k, const void* v, void* out, float* lse,
-                                const int* cu_seqlens, int batch, long long total_tokens, int hq, int hkv, int head_dim,
-                                float scale, int window, const float* alibi_slopes, int dtype, cudaStream_t stream) {
-  if (batch <= 0 || total_tokens <= 0) return 0;
-  if (hq % hkv || (dtype != CB_BF16 && dtype != CB_F16) || cu_seqlens == nullptr || window < 0)
+  const bool packed = cu_seqlens != nullptr;
+  if ((dtype != CB_BF16 && dtype != CB_F16) || hkv <= 0 || hq % hkv || (head_dim != 64 && head_dim != 128) ||
+      (!packed && causal && seqlen_q != seqlen_k) || window < 0 || ((window > 0 || alibi) && !(packed && causal)) ||
+      (o_state ? (packed || lse == nullptr) : has_prev != 0))
     return (int)cudaErrorInvalidValue;
-  if (head_dim == 128)
-    return launch_flash_fwd<128>(q, k, v, out, lse, batch, 0, 0, hq, hkv, 1, scale, dtype, stream, cu_seqlens,
-                                 total_tokens, nullptr, 0, window, alibi_slopes);
-  if (head_dim == 64)
-    return launch_flash_fwd<64>(q, k, v, out, lse, batch, 0, 0, hq, hkv, 1, scale, dtype, stream, cu_seqlens,
-                                total_tokens, nullptr, 0, window, alibi_slopes);
-  return (int)cudaErrorInvalidValue;
+  if (batch <= 0 || (packed ? total_tokens <= 0 : seqlen_q <= 0)) return 0;
+  return (head_dim == 128 ? launch_flash_fwd<128> : launch_flash_fwd<64>)(
+      q, k, v, out, lse, batch, seqlen_q, seqlen_k, hq, hkv, causal, scale, dtype, stream, cu_seqlens, total_tokens,
+      o_state, has_prev, window, alibi);
 }
 
 // Backward of cb_flash_attn_fwd for self attention (seqlen_q == seqlen_k).  q / out / dout / dq [T, hq, D], k / v / dk /
 // dv [T, hkv, D], lse [T, hq] fp32 from the forward.  Workspaces: delta [T, hq] fp32 and dq_acc [T, hq, D] fp32 (this
-// function zeroes dq_acc).  Requirements as the forward; head_dim 128 (64 also instantiated).
+// function zeroes dq_acc).  dtype and GQA as the forward; head_dim 128.
 int cb_flash_attn_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
                       void* dq, void* dk, void* dv, float* delta, float* dq_acc, int batch, int seqlen, int hq, int hkv,
                       int head_dim, int causal, float scale, int dtype, const int* cu_seqlens, long long total_tokens,
                       cudaStream_t stream) {
+  if (!bwd_args_ok(hq, hkv, head_dim, dtype)) return (int)cudaErrorInvalidValue;
   // cu_seqlens != null: packed batch of `total_tokens` rows (seqlen ignored); else `batch` sequences of `seqlen`
   if (batch <= 0 || (cu_seqlens ? total_tokens <= 0 : seqlen <= 0)) return 0;
-  if (hq % hkv || head_dim != 128) return (int)cudaErrorInvalidValue;
-  if (dtype != CB_BF16 && dtype != CB_F16) return (int)cudaErrorInvalidValue;
   const long long rows = (cu_seqlens ? total_tokens : (long long)batch * seqlen) * hq;
   const long long n = rows * head_dim;
   cudaError_t e = cudaMemsetAsync(dq_acc, 0, (size_t)n * sizeof(float), stream);
   if (e != cudaSuccess) return (int)e;
-  const int wpb = 8;
-  if (dtype == CB_BF16)
-    flash_bwd_delta_kernel<__nv_bfloat16><<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(
-        (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta, rows, head_dim);
-  else
-    flash_bwd_delta_kernel<__half><<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(
-        (const __half*)out, (const __half*)dout, delta, rows, head_dim);
-  int rc = launch_flash_bwd<128>(q, k, v, dout, lse, delta, dq_acc, dk, dv, batch, seqlen, hq, hkv, causal, scale, dtype,
-                                 stream, cu_seqlens, total_tokens);
+  int rc = launch_flash_delta(out, dout, delta, rows, head_dim, dtype, stream);
+  if (rc) return rc;
+  rc = launch_flash_bwd<128>(q, k, v, dout, lse, delta, dq_acc, dk, dv, batch, seqlen, hq, hkv, causal, scale, dtype,
+                             stream, cu_seqlens, total_tokens);
   if (rc) return rc;
   const unsigned blocks = (unsigned)((n / 8 + 255) / 256);
   if (dtype == CB_BF16) flash_bwd_cast_dq_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(dq_acc, (__nv_bfloat16*)dq, n);
@@ -840,34 +832,20 @@ int cb_flash_attn_bwd(const void* q, const void* k, const void* v, const void* o
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Blockwise entry points for fused ring (context-parallel) attention.  One launch = the queries of this rank against ONE
+// Blockwise attention for fused ring (context-parallel) attention.  One launch = the queries of this rank against ONE
 // key/value block that may live in a PEER's memory (k / v are then peer-mapped symmetric-buffer addresses: the TMA
 // loads of the main loop pull the tiles over NVLink, GQA heads only, no staging copy).
-//   forward : the online-softmax state (o_state fp32, lse) is carried from launch to launch inside the kernel
-//             (`has_prev`), which replaces the reference's per-hop `_rescale_out_lse` pass (`layer/attn.py:376-403`);
+//   forward : cb_flash_attn_fwd in block mode.  The online-softmax state (o_state fp32, lse) is carried from launch to
+//             launch inside the kernel (`has_prev`), which replaces the reference's per-hop `_rescale_out_lse` pass
+//             (`layer/attn.py:376-403`);
 //   backward: dQ accumulates in the local fp32 `dq_acc` (not zeroed here), dK / dV are reduced straight into the block
 //             owner's fp32 accumulators (`dk_acc` / `dv_acc`, peer pointers) - the reference circulates fp32 dKV
 //             buffers around the ring instead (`layer/attn.py:1066-1163`).  `delta` = rowsum(dO o O) is an input.
-int cb_flash_attn_block_fwd(const void* q, const void* k, const void* v, float* o_state, float* lse, int rows, int hq,
-                            int hkv, int head_dim, int causal, int has_prev, float scale, int dtype, cudaStream_t stream) {
-  if (rows <= 0) return 0;
-  if (hq % hkv || (dtype != CB_BF16 && dtype != CB_F16) || o_state == nullptr || lse == nullptr)
-    return (int)cudaErrorInvalidValue;
-  if (head_dim == 128)
-    return launch_flash_fwd<128>(q, k, v, nullptr, lse, 1, rows, rows, hq, hkv, causal, scale, dtype, stream, nullptr, 0,
-                                 o_state, has_prev);
-  if (head_dim == 64)
-    return launch_flash_fwd<64>(q, k, v, nullptr, lse, 1, rows, rows, hq, hkv, causal, scale, dtype, stream, nullptr, 0,
-                                o_state, has_prev);
-  return (int)cudaErrorInvalidValue;
-}
-
 int cb_flash_attn_block_bwd(const void* q, const void* k, const void* v, const void* dout, const float* lse,
                             const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int rows, int hq, int hkv,
                             int head_dim, int causal, float scale, int dtype, cudaStream_t stream) {
+  if (!bwd_args_ok(hq, hkv, head_dim, dtype) || !dq_acc || !dk_acc || !dv_acc) return (int)cudaErrorInvalidValue;
   if (rows <= 0) return 0;
-  if (hq % hkv || head_dim != 128 || (dtype != CB_BF16 && dtype != CB_F16) || !dq_acc || !dk_acc || !dv_acc)
-    return (int)cudaErrorInvalidValue;
   return launch_flash_bwd<128>(q, k, v, dout, lse, delta, dq_acc, nullptr, nullptr, 1, rows, hq, hkv, causal, scale, dtype,
                                stream, nullptr, 0, dk_acc, dv_acc);
 }
@@ -875,17 +853,9 @@ int cb_flash_attn_block_bwd(const void* q, const void* k, const void* v, const v
 // delta[t, h] = sum_d dO o O for `rows` (token, head) rows of width head_dim
 int cb_flash_attn_delta(const void* out, const void* dout, float* delta, long long rows, int head_dim, int dtype,
                         cudaStream_t stream) {
+  if (dtype != CB_BF16 && dtype != CB_F16) return (int)cudaErrorInvalidValue;
   if (rows <= 0) return 0;
-  const int wpb = 8;
-  if (dtype == CB_BF16)
-    flash_bwd_delta_kernel<__nv_bfloat16><<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(
-        (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta, rows, head_dim);
-  else if (dtype == CB_F16)
-    flash_bwd_delta_kernel<__half><<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(
-        (const __half*)out, (const __half*)dout, delta, rows, head_dim);
-  else
-    return (int)cudaErrorInvalidValue;
-  return (int)cudaGetLastError();
+  return launch_flash_delta(out, dout, delta, rows, head_dim, dtype, stream);
 }
 
 }  // extern "C"

@@ -16,7 +16,8 @@ import torch.distributed as dist
 from torch.distributed import ProcessGroup
 
 from ... import ops
-from ...ops.attention import AttnMaskType, attention_with_lse_ref
+from ...ops.attention import AttnMaskType
+from ...ops.flash_attn_native import _block_bwd, _block_fwd
 from ...parallel import comm
 from .utils import RingComm
 
@@ -95,82 +96,6 @@ def _merge(out: Optional[torch.Tensor], lse: Optional[torch.Tensor], blk_out: to
     w_old = torch.nan_to_num(w_old, nan=0.0)
     w_new = torch.nan_to_num(w_new, nan=0.0)
     return out * w_old + blk_out.float() * w_new, new_lse
-
-
-def _to_bhsd(x: torch.Tensor, batch: int, rep: int = 1) -> torch.Tensor:
-    T, H, D = x.shape
-    xb = x.view(batch, T // batch, H, D).transpose(1, 2)
-    return xb if rep == 1 else xb.repeat_interleave(rep, dim=1)
-
-
-def _lib_flash_ok(q: torch.Tensor) -> bool:
-    return q.is_cuda and q.dtype in (torch.float16, torch.bfloat16) and q.shape[-1] <= 256 and q.shape[-1] % 8 == 0 \
-        and hasattr(torch.ops.aten, "_scaled_dot_product_flash_attention")
-
-
-def _block_fwd(q, k, v, batch, causal, scale):
-    """One attention block returning (out [T,Hq,D], lse [T,Hq] fp32).  CUDA: the library flash kernel through aten (it
-    returns the log-sum-exp needed by the online-softmax merge) until the wgmma kernel lands; CPU: explicit softmax."""
-    from ...ops import flash_attn_native as fa
-
-    if q.is_cuda and fa.supported(q, k, v, None):
-        return fa.flash_attention_with_lse(q, k, v, batch=batch, causal=causal, scale=scale)
-    if _lib_flash_ok(q) and (not causal or q.shape[0] == k.shape[0]):
-        g = q.shape[1] // k.shape[1]
-        res = torch.ops.aten._scaled_dot_product_flash_attention(_to_bhsd(q, batch), _to_bhsd(k, batch, g),
-                                                                 _to_bhsd(v, batch, g), 0.0, causal, False, scale=scale)
-        out, lse = res[0], res[1]                       # [B,H,S,D], [B,H,S]
-        return out.transpose(1, 2).reshape(q.shape), lse.transpose(1, 2).reshape(q.shape[0], q.shape[1])
-    return attention_with_lse_ref(q, k, v, batch=batch, causal=causal, scale=scale)
-
-
-def _block_bwd(do, q, k, v, o, lse, batch, causal, scale):
-    """Gradients of one attention block GIVEN the final (merged) lse: p = exp(s - lse_final)."""
-    from ...ops import flash_attn_native as fa
-
-    if q.is_cuda and fa.supported(q, k, v, None) and hasattr(fa, "flash_attention_bwd"):
-        return fa.flash_attention_bwd(do, q, k, v, o, lse, batch=batch, causal=causal, scale=scale)
-    if _lib_flash_ok(q) and (not causal or q.shape[0] == k.shape[0]) \
-            and hasattr(torch.ops.aten, "_scaled_dot_product_flash_attention_backward"):
-        Hq, Hkv = q.shape[1], k.shape[1]
-        g = Hq // Hkv
-        Sq, Sk = q.shape[0] // batch, k.shape[0] // batch
-        qb, kb, vb = _to_bhsd(q, batch), _to_bhsd(k, batch, g), _to_bhsd(v, batch, g)
-        ob, dob = _to_bhsd(o.to(q.dtype), batch), _to_bhsd(do.to(q.dtype), batch)
-        lb = lse.view(batch, Sq, Hq).transpose(1, 2).contiguous().float()
-        z = torch.zeros((), dtype=torch.int64, device=q.device)
-        dq, dk, dv = torch.ops.aten._scaled_dot_product_flash_attention_backward(
-            dob.contiguous(), qb.contiguous(), kb.contiguous(), vb.contiguous(), ob.contiguous(), lb, None, None, Sq, Sk,
-            0.0, causal, z, z, scale=scale)
-        dq = dq.transpose(1, 2).reshape(q.shape).float()
-        dk = dk.float().view(batch, Hkv, g, Sk, -1).sum(2).transpose(1, 2).reshape(k.shape)
-        dv = dv.float().view(batch, Hkv, g, Sk, -1).sum(2).transpose(1, 2).reshape(v.shape)
-        return dq, dk, dv
-    T, Hq, D = q.shape
-    Tk, Hkv = k.shape[0], k.shape[1]
-    Sq, Sk, g = T // batch, Tk // batch, Hq // Hkv
-    qb = q.view(batch, Sq, Hq, D).transpose(1, 2).float()
-    kb = k.view(batch, Sk, Hkv, D).transpose(1, 2).float().repeat_interleave(g, 1)
-    vb = v.view(batch, Sk, Hkv, D).transpose(1, 2).float().repeat_interleave(g, 1)
-    dob = do.view(batch, Sq, Hq, D).transpose(1, 2).float()
-    ob = o.view(batch, Sq, Hq, D).transpose(1, 2).float()
-    lb = lse.view(batch, Sq, Hq).transpose(1, 2).float()
-    s = torch.matmul(qb, kb.transpose(-1, -2)) * scale
-    if causal:
-        m = torch.ones(Sq, Sk, dtype=torch.bool, device=q.device).tril(diagonal=Sk - Sq)
-        s = s.masked_fill(~m, float("-inf"))
-    p = torch.exp(s - lb.unsqueeze(-1))
-    p = torch.nan_to_num(p, nan=0.0)
-    dv = torch.matmul(p.transpose(-1, -2), dob)
-    dp = torch.matmul(dob, vb.transpose(-1, -2))
-    delta = (dob * ob).sum(-1, keepdim=True)
-    ds = p * (dp - delta) * scale
-    dq = torch.matmul(ds, kb)
-    dk = torch.matmul(ds.transpose(-1, -2), qb)
-    dq = dq.transpose(1, 2).reshape(T, Hq, D)
-    dk = dk.view(batch, Hkv, g, Sk, D).sum(2).transpose(1, 2).reshape(Tk, Hkv, D)
-    dv = dv.view(batch, Hkv, g, Sk, D).sum(2).transpose(1, 2).reshape(Tk, Hkv, D)
-    return dq, dk, dv
 
 
 def _p2p_gather_kv(kv: torch.Tensor, sp_group) -> Optional[torch.Tensor]:

@@ -30,7 +30,6 @@ published" and, in backward, "everybody's reductions have landed".
 """
 from __future__ import annotations
 
-import ctypes
 import math
 import os
 from typing import Dict, Optional, Tuple
@@ -39,21 +38,13 @@ import torch
 import torch.distributed as dist
 
 from ...kernel import loader
-from ...ops._dtypes import code
+from ...ops import flash_attn_native as fa
 from ...parallel import comm
 
 __all__ = ["available", "ring_attention_fused", "stats"]
 
 stats = {"fwd_blocks": 0, "bwd_blocks": 0, "layers_fwd": 0, "layers_bwd": 0}
 _workspaces: Dict[tuple, "_RingWorkspace"] = {}
-_lib = None
-
-
-def _get_lib():
-    global _lib
-    if _lib is None:
-        _lib = loader.load("cb200_attn")
-    return _lib
 
 
 def available(q: torch.Tensor, k: torch.Tensor, sp_group, batch: int) -> bool:
@@ -124,10 +115,6 @@ def _visit_order(r: int, sp: int):
     return [(r - step) % sp for step in range(sp)]
 
 
-def _p(addr: int) -> ctypes.c_void_p:
-    return ctypes.c_void_p(addr)
-
-
 class _FusedRing(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, k, v, sp_group, batch, scale):
@@ -170,9 +157,6 @@ class _FusedRing(torch.autograd.Function):
             pull(1)
         o_state = torch.empty(T, Hq, D, dtype=torch.float32, device=q.device)
         lse = torch.empty(T, Hq, dtype=torch.float32, device=q.device)
-        lib = _get_lib()
-        dt = code(q.dtype)
-        stream = loader.stream_ptr()
         row_q, row_kv, row_o, row_l = Hq * D * es, Hkv * D * es, Hq * D * 4, Hq * 4
         started = [[False, False] for _ in range(batch)]
         for i, src in enumerate(order):
@@ -187,12 +171,10 @@ class _FusedRing(torch.autograd.Function):
                 for qh, kh, causal in _blocks(r, src):
                     q_off = b * S + qh * half
                     k_off = b * S + kh * half
-                    rc = lib.cb_flash_attn_block_fwd(
-                        _p(q.data_ptr() + q_off * row_q), _p(base + k_off * row_kv),
-                        _p(base + (kv_elems * es) + k_off * row_kv), _p(o_state.data_ptr() + q_off * row_o),
-                        _p(lse.data_ptr() + q_off * row_l), half, Hq, Hkv, D, int(causal), int(started[b][qh]),
-                        ctypes.c_float(scale), dt, stream)
-                    loader.check(rc, "flash_attn_block_fwd")
+                    fa.flash_block_fwd(
+                        q.data_ptr() + q_off * row_q, base + k_off * row_kv, base + (kv_elems * es) + k_off * row_kv,
+                        o_state.data_ptr() + q_off * row_o, lse.data_ptr() + q_off * row_l, half, Hq, Hkv, D, causal,
+                        started[b][qh], scale, q.dtype)
                     started[b][qh] = True
                     stats["fwd_blocks"] += 1
             consumed[i] = torch.cuda.Event()
@@ -219,18 +201,13 @@ class _FusedRing(torch.autograd.Function):
         buf = ws.kv[ws.toggle]
         ws.toggle ^= 1
         dout = dout.contiguous()
-        lib = _get_lib()
-        dt = code(q.dtype)
-        stream = loader.stream_ptr()
         pub = buf.tensor[: 2 * kv_elems * es].view(q.dtype).view(2, T, Hkv, D)
         pub[0].copy_(k)
         pub[1].copy_(v)
         acc = ws.dkv.tensor[: 2 * kv_elems * 4].view(torch.float32)
         acc.zero_()
         ws.barrier()                                  # K/V published and accumulators cleared everywhere
-        delta = torch.empty(T, Hq, dtype=torch.float32, device=q.device)
-        loader.check(lib.cb_flash_attn_delta(loader.ptr(out), loader.ptr(dout), loader.ptr(delta),
-                                             ctypes.c_longlong(T * Hq), D, dt, stream), "flash_attn_delta")
+        delta = fa.flash_delta(out, dout)
         dq_acc = torch.zeros(T, Hq, D, dtype=torch.float32, device=q.device)
         row_q, row_kv, row_dq, row_l, row_acc = Hq * D * es, Hkv * D * es, Hq * D * 4, Hq * 4, Hkv * D * 4
         for src in _visit_order(r, sp):
@@ -240,14 +217,12 @@ class _FusedRing(torch.autograd.Function):
                 for qh, kh, causal in _blocks(r, src):
                     q_off = b * S + qh * half
                     k_off = b * S + kh * half
-                    rc = lib.cb_flash_attn_block_bwd(
-                        _p(q.data_ptr() + q_off * row_q), _p(base + k_off * row_kv),
-                        _p(base + kv_elems * es + k_off * row_kv), _p(dout.data_ptr() + q_off * row_q),
-                        _p(lse.data_ptr() + q_off * row_l), _p(delta.data_ptr() + q_off * row_l),
-                        _p(dq_acc.data_ptr() + q_off * row_dq), _p(acc_base + k_off * row_acc),
-                        _p(acc_base + kv_elems * 4 + k_off * row_acc), half, Hq, Hkv, D, int(causal),
-                        ctypes.c_float(scale), dt, stream)
-                    loader.check(rc, "flash_attn_block_bwd")
+                    fa.flash_block_bwd(
+                        q.data_ptr() + q_off * row_q, base + k_off * row_kv, base + kv_elems * es + k_off * row_kv,
+                        dout.data_ptr() + q_off * row_q, lse.data_ptr() + q_off * row_l,
+                        delta.data_ptr() + q_off * row_l, dq_acc.data_ptr() + q_off * row_dq,
+                        acc_base + k_off * row_acc, acc_base + kv_elems * 4 + k_off * row_acc, half, Hq, Hkv, D,
+                        causal, scale, q.dtype)
                     stats["bwd_blocks"] += 1
         loader.launch_counter.add("ring_attn_block_bwd", sp * batch * 2 + batch)
         stats["layers_bwd"] += 1

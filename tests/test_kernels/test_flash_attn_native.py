@@ -199,21 +199,19 @@ def test_attention_frontend_packed_uses_native_kernels():
         assert (got.float() - ref).abs().max().item() <= 3e-2 * ref.abs().max().item() + 1e-6
 
 
+@pytest.mark.parametrize("D", [64, 128])
 @pytest.mark.parametrize("rows,Hq,Hkv", [(256, 8, 2), (512, 4, 4), (1024, 8, 8)])
 @pytest.mark.parametrize("big_second", [False, True])
-def test_flash_block_mode_state_carry(rows, Hq, Hkv, big_second):
+def test_flash_block_mode_state_carry(rows, Hq, Hkv, big_second, D):
     """Block mode (ring attention building block): the keys are visited as two blocks by two launches; the second
     launch resumes from the fp32 (output, LSE) state of the first.  `big_second` scales the second block's keys so that
-    its scores dominate (the carried accumulator has to be rescaled inside the kernel)."""
-    import ctypes
+    its scores dominate (the carried accumulator has to be rescaled inside the kernel).  Both head dims the block
+    forward accepts."""
     import math
 
-    from colossalai_b200.kernel import loader
-    from colossalai_b200.ops._dtypes import code
-    from colossalai_b200.ops.attention import attention_with_lse_ref
+    from colossalai_b200.ops import flash_attn_native as fa
 
-    D, dtype = 128, torch.bfloat16
-    lib = loader.load("cb200_attn")
+    dtype = torch.bfloat16
     torch.manual_seed(7)
     q = torch.randn(rows, Hq, D, device="cuda", dtype=dtype)
     k = torch.randn(2 * rows, Hkv, D, device="cuda", dtype=dtype)
@@ -224,10 +222,8 @@ def test_flash_block_mode_state_carry(rows, Hq, Hkv, big_second):
     lse = torch.empty(rows, Hq, device="cuda", dtype=torch.float32)
     scale = 1.0 / math.sqrt(D)
     for blk, (causal, has_prev) in enumerate([(0, 0), (1, 1)]):
-        rc = lib.cb_flash_attn_block_fwd(loader.ptr(q), loader.ptr(k[blk * rows:]), loader.ptr(v[blk * rows:]),
-                                         loader.ptr(o_state), loader.ptr(lse), rows, Hq, Hkv, D, causal, has_prev,
-                                         ctypes.c_float(scale), code(dtype), loader.stream_ptr())
-        loader.check(rc, "flash_attn_block_fwd")
+        fa.flash_block_fwd(q.data_ptr(), k[blk * rows:].data_ptr(), v[blk * rows:].data_ptr(), o_state.data_ptr(),
+                           lse.data_ptr(), rows, Hq, Hkv, D, causal, has_prev, scale, dtype)
     torch.cuda.synchronize()
     # oracle: queries are the LAST `rows` positions of a 2*rows sequence (first block fully visible, second causal)
     g = Hq // Hkv
@@ -242,3 +238,94 @@ def test_flash_block_mode_state_carry(rows, Hq, Hkv, big_second):
     ref_lse = torch.logsumexp(sc, -1).transpose(0, 1)
     torch.testing.assert_close(lse, ref_lse, atol=3e-3, rtol=3e-3)
     torch.testing.assert_close(o_state, ref, atol=2e-2, rtol=2e-2)
+
+
+@pytest.mark.parametrize("rows,Hq,Hkv", [(256, 8, 2), (512, 4, 4), (200, 8, 2)])
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_flash_block_mode_backward(rows, Hq, Hkv, dtype):
+    """Block-mode backward (ring attention building block) on one GPU: the queries are the last `rows` positions of a
+    2*rows sequence, the keys two blocks (the first fully visible, the second causal).  Each block's backward adds into
+    the same fp32 dQ / dK / dV accumulators, with the merged forward's LSE and delta."""
+    from colossalai_b200.ops import flash_attn_native as fa
+    from colossalai_b200.ops.attention import attention_with_lse_ref
+
+    D = 128
+    scale = D ** -0.5
+    torch.manual_seed(8)
+    q = torch.randn(rows, Hq, D, device="cuda", dtype=dtype)
+    k = torch.randn(2 * rows, Hkv, D, device="cuda", dtype=dtype)
+    v = torch.randn(2 * rows, Hkv, D, device="cuda", dtype=dtype)
+    dout = torch.randn(rows, Hq, D, device="cuda", dtype=dtype)
+    o_state = torch.empty(rows, Hq, D, device="cuda", dtype=torch.float32)
+    lse = torch.empty(rows, Hq, device="cuda", dtype=torch.float32)
+    blocks = [(0, False), (1, True)]                      # (key block, causal)
+    for blk, causal in blocks:
+        fa.flash_block_fwd(q.data_ptr(), k[blk * rows:].data_ptr(), v[blk * rows:].data_ptr(), o_state.data_ptr(),
+                           lse.data_ptr(), rows, Hq, Hkv, D, causal, blk > 0, scale, dtype)
+    delta = fa.flash_delta(o_state.to(dtype), dout)
+    dq_acc = torch.zeros(rows, Hq, D, device="cuda", dtype=torch.float32)
+    dk_acc = torch.zeros(2 * rows, Hkv, D, device="cuda", dtype=torch.float32)
+    dv_acc = torch.zeros_like(dk_acc)
+    for blk, causal in blocks:
+        fa.flash_block_bwd(q.data_ptr(), k[blk * rows:].data_ptr(), v[blk * rows:].data_ptr(), dout.data_ptr(),
+                           lse.data_ptr(), delta.data_ptr(), dq_acc.data_ptr(), dk_acc[blk * rows:].data_ptr(),
+                           dv_acc[blk * rows:].data_ptr(), rows, Hq, Hkv, D, causal, scale, dtype)
+    qf, kf, vf = (t.float().requires_grad_(True) for t in (q, k, v))
+    ref_o, _ = attention_with_lse_ref(qf, kf, vf, batch=1, causal=True, scale=scale)     # bottom-right causal
+    ref_o.backward(dout.float())
+    torch.cuda.synchronize()
+    for name, got, ref in (("dq", dq_acc, qf.grad), ("dk", dk_acc, kf.grad), ("dv", dv_acc, vf.grad)):
+        err = (got - ref).abs().max().item()
+        scale_ = ref.abs().max().item()
+        assert err <= 2e-2 * scale_ + 1e-3, f"{name}: max err {err:.4g} vs max |ref| {scale_:.4g}"
+        assert (got - ref).mean().abs().item() <= 2e-3 * ref.abs().mean().item() + 1e-5, name
+
+
+def test_flash_fwd_launcher_rejects_out_of_envelope():
+    """The forward launcher validates before anything else, empty problems included: every call outside its envelope
+    fails with cudaErrorInvalidValue (1) and writes nothing."""
+    from colossalai_b200.ops import flash_attn_native as fa
+
+    T, Hq, Hkv, D, dtype = 256, 4, 2, 128, torch.bfloat16
+    torch.manual_seed(9)
+    q = torch.randn(T, Hq, D, device="cuda", dtype=dtype)
+    k = torch.randn(T, Hkv, D, device="cuda", dtype=dtype)
+    v = torch.randn(T, Hkv, D, device="cuda", dtype=dtype)
+    out = torch.full_like(q, float("nan"))
+    lse = torch.full((T, Hq), float("nan"), device="cuda")
+    o_state = torch.full((T, Hq, D), float("nan"), device="cuda")
+    cu = torch.tensor([0, 100, T], device="cuda", dtype=torch.int32)
+    slopes = torch.ones(Hq, device="cuda")
+    uniform = dict(q=q.data_ptr(), k=k.data_ptr(), v=v.data_ptr(), out=out.data_ptr(), lse=lse.data_ptr(), batch=1,
+                   seqlen_q=T, seqlen_k=T, hq=Hq, hkv=Hkv, d=D, causal=True, scale=D ** -0.5, dtype=dtype)
+    packed = dict(uniform, batch=2, seqlen_q=0, seqlen_k=0, cu_seqlens=cu.data_ptr(), total_tokens=T)
+    block = dict(uniform, out=0, o_state=o_state.data_ptr())
+    rejected = {
+        "fp32": dict(uniform, dtype=torch.float32),
+        "head_dim 96": dict(uniform, d=96),
+        "hq % hkv != 0": dict(uniform, hq=3),
+        "hkv 0": dict(uniform, hkv=0),
+        "causal, seqlen_q != seqlen_k": dict(uniform, seqlen_k=T // 2),
+        "window without cu_seqlens": dict(uniform, window=64),
+        "alibi without cu_seqlens": dict(uniform, alibi=slopes.data_ptr()),
+        "negative window": dict(packed, window=-1),
+        "window, not causal": dict(packed, causal=False, window=64),
+        "alibi, not causal": dict(packed, causal=False, alibi=slopes.data_ptr()),
+        "block mode, null lse": dict(block, lse=0),
+        "block mode with cu_seqlens": dict(block, cu_seqlens=cu.data_ptr(), total_tokens=T),
+        "has_prev without o_state": dict(uniform, has_prev=True),
+        "empty, head_dim 96": dict(uniform, batch=0, d=96),
+        "empty packed, fp32": dict(packed, total_tokens=0, dtype=torch.float32),
+    }
+    for name, args in rejected.items():
+        with pytest.raises(RuntimeError, match=r"CUDA error 1$"):
+            fa._fwd(name, **args)
+    torch.cuda.synchronize()
+    for t in (out, lse, o_state):
+        assert torch.isnan(t).all(), "a rejected call wrote its output"
+    # the same buffers are written by calls inside the envelope
+    fa._fwd("uniform", **uniform)
+    fa._fwd("block", **block)
+    torch.cuda.synchronize()
+    for t in (out, lse, o_state):
+        assert torch.isfinite(t).all()
