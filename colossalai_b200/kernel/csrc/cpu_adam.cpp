@@ -51,16 +51,19 @@ inline uint16_t f32_to_f16(float f) {
   uint32_t man = u & 0x7fffffu;
   if (((u >> 23) & 0xff) == 0xff) return (uint16_t)(sign | 0x7c00u | (man ? 0x200u : 0));
   if (exp >= 31) return (uint16_t)(sign | 0x7c00u);
+  // round to nearest, ties to even (a carry out of the mantissa bumps the exponent, up to inf)
   if (exp <= 0) {
     if (exp < -10) return (uint16_t)sign;
     man |= 0x800000u;
     const int shift = 14 - exp;
     uint32_t r = man >> shift;
-    if ((man >> (shift - 1)) & 1u) r += 1;
+    const uint32_t rem = man & ((1u << shift) - 1u), half = 1u << (shift - 1);
+    if (rem > half || (rem == half && (r & 1u))) r += 1;
     return (uint16_t)(sign | r);
   }
   uint32_t r = (uint32_t)(exp << 10) | (man >> 13);
-  if (man & 0x1000u) r += 1;
+  const uint32_t rem = man & 0x1fffu;
+  if (rem > 0x1000u || (rem == 0x1000u && (r & 1u))) r += 1;
   return (uint16_t)(sign | r);
 }
 

@@ -196,6 +196,28 @@ __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_sgd_kernel(const int
 }
 
 // ------------------------------------------------------------------------------------------------ norms
+// The max norm propagates NaN like torch's `vector_norm(ord=inf)`: `fmaxf` (PTX `max.f32`) returns the other
+// operand when one is NaN, so a NaN gradient would report a finite norm.  `max.NaN.f32` (sm_80+) returns NaN.
+CB_DEVICE float nan_max(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+CB_DEVICE float block_max_nan(float v, float* smem) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = nan_max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if (nwarps == 1) return v;
+  __syncthreads();
+  if (lane == 0) smem[warp] = v;
+  __syncthreads();
+  v = lane < nwarps ? smem[lane] : 0.f;   // every partial is an absolute value (>= 0) or NaN
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = nan_max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
 // partial[chunk] = sum (or max) over the chunk of x^2 (|x|); `which`: 0 = param, 1 = grad, 2 = m (update buffer)
 __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_norm_partial_kernel(const int64_t* __restrict__ tbl,
                                                                                int num_tensors, int which,
@@ -218,7 +240,7 @@ __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_norm_partial_kernel(
     if (mis) head = min(n, (int64_t)((16 - mis) / esz));
     for (int64_t j = threadIdx.x; j < head; j += blockDim.x) {
       const float x = ld_any(src, dt, off + j);
-      acc = use_max ? fmaxf(acc, fabsf(x)) : acc + x * x;
+      acc = use_max ? nan_max(acc, fabsf(x)) : acc + x * x;
     }
     const int64_t nvec = (n - head) / per;
     const uint4* vp = reinterpret_cast<const uint4*>(base + head * esz);
@@ -247,22 +269,22 @@ __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_norm_partial_kernel(
           a0 = __low2float(h0); a1 = __high2float(h0); b0 = __low2float(h1); b1 = __high2float(h1);
         }
         if (use_max) {
-          acc = fmaxf(acc, fmaxf(fabsf(a0), fabsf(a1)));
-          acc2 = fmaxf(acc2, fmaxf(fabsf(b0), fabsf(b1)));
+          acc = nan_max(acc, nan_max(fabsf(a0), fabsf(a1)));
+          acc2 = nan_max(acc2, nan_max(fabsf(b0), fabsf(b1)));
         } else {
           acc += a0 * a0 + a1 * a1;
           acc2 += b0 * b0 + b1 * b1;
         }
       }
     }
-    acc = use_max ? fmaxf(acc, acc2) : acc + acc2;
+    acc = use_max ? nan_max(acc, acc2) : acc + acc2;
     for (int64_t j = head + nvec * per + threadIdx.x; j < n; j += blockDim.x) {     // scalar tail
       const float x = ld_any(src, dt, off + j);
-      acc = use_max ? fmaxf(acc, fabsf(x)) : acc + x * x;
+      acc = use_max ? nan_max(acc, fabsf(x)) : acc + x * x;
     }
   }
   if (use_max) {
-    acc = block_max(acc, red);
+    acc = block_max_nan(acc, red);
   } else {
     float a[1] = {acc};
     block_sum<1>(a, red);
@@ -280,8 +302,8 @@ __global__ void __launch_bounds__(1024) norm_finalize_kernel(const float* __rest
   if (blockIdx.x == 0) {
     float acc = 0.f;
     for (int64_t i = threadIdx.x; i < n_chunks; i += blockDim.x)
-      acc = use_max ? fmaxf(acc, partial[i]) : acc + partial[i];
-    if (use_max) acc = block_max(acc, red);
+      acc = use_max ? nan_max(acc, partial[i]) : acc + partial[i];
+    if (use_max) acc = block_max_nan(acc, red);
     else { float a[1] = {acc}; block_sum<1>(a, red); acc = a[0]; }
     if (threadIdx.x == 0) out[0] = acc;   // squared L2 norm (or max): python takes the sqrt after cross-rank reduce
   } else if (per_tensor) {
@@ -290,8 +312,8 @@ __global__ void __launch_bounds__(1024) norm_finalize_kernel(const float* __rest
       const int64_t c1 = (t + 1 < num_tensors) ? tbl[(int64_t)(t + 1) * TBL_COLS + 7] : n_chunks;
       float acc = 0.f;
       for (int64_t i = c0 + threadIdx.x; i < c1; i += blockDim.x)
-        acc = use_max ? fmaxf(acc, partial[i]) : acc + partial[i];
-      if (use_max) acc = block_max(acc, red);
+        acc = use_max ? nan_max(acc, partial[i]) : acc + partial[i];
+      if (use_max) acc = block_max_nan(acc, red);
       else { float a[1] = {acc}; block_sum<1>(a, red); acc = a[0]; }
       if (threadIdx.x == 0) per_tensor[t] = acc;
       __syncthreads();
@@ -345,7 +367,8 @@ __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_lamb_stage1_kernel(c
   }
 }
 
-// stage 2: p -= lr * trust_ratio[t] * u   with trust = ||p|| / ||u|| (1 when either is 0)
+// stage 2: p -= lr * trust_ratio[t] * u   with trust = ||p|| / ||u|| (1 when either is 0).  Null norm pointers mean
+// no trust ratio (ratio 1): the reference applies it only with `use_nvlamb` or a non-zero weight decay.
 __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_lamb_stage2_kernel(const int64_t* __restrict__ tbl,
                                                                                int num_tensors, float lr,
                                                                                const float* __restrict__ p_norm_sq,
@@ -358,8 +381,11 @@ __global__ void __launch_bounds__(OPT_THREADS) multi_tensor_lamb_stage2_kernel(c
   const int64_t off = (chunk - t.chunk0) * CHUNK;
   if (off >= t.n) return;
   const int64_t n = min((int64_t)CHUNK, t.n - off);
-  const float pn = sqrtf(p_norm_sq[ti]), un = sqrtf(u_norm_sq[ti]);
-  const float ratio = (pn > 0.f && un > 0.f) ? pn / un : 1.f;
+  float ratio = 1.f;
+  if (p_norm_sq && u_norm_sq) {
+    const float pn = sqrtf(p_norm_sq[ti]), un = sqrtf(u_norm_sq[ti]);
+    if (pn > 0.f && un > 0.f) ratio = pn / un;
+  }
   for (int64_t j = threadIdx.x; j < n; j += blockDim.x) {
     float p = ld_any(t.p, t.pd, off + j);
     p -= lr * ratio * ld_any(t.g, t.gd, off + j);

@@ -72,6 +72,7 @@ class FusedAdam(torch.optim.Optimizer):
         inv_scale = 1.0 / div_scale if div_scale > 0 else 1.0
         for group in self.param_groups:
             ps, gs, ms, vs = [], [], [], []
+            staged = []         # (param, contiguous copy stepped in its place): written back after the step
             group["step"] = group.get("step", 0) + 1
             beta1, beta2 = group["betas"]
             for p in group["params"]:
@@ -83,17 +84,24 @@ class FusedAdam(torch.optim.Optimizer):
                 if len(st) == 0:
                     st["exp_avg"] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.contiguous_format)
                     st["exp_avg_sq"] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.contiguous_format)
-                ps.append(p.data if p.data.is_contiguous() else p.data.contiguous())
+                if p.data.is_contiguous():
+                    ps.append(p.data)
+                else:
+                    ps.append(p.data.contiguous())
+                    staged.append((p, ps[-1]))
                 gs.append(p.grad.data if p.grad.data.is_contiguous() else p.grad.data.contiguous())
                 ms.append(st["exp_avg"])
                 vs.append(st["exp_avg_sq"])
             if not ps:
                 continue
             if use_native(ps[0]):
-                mt.adam(self._table(ps, gs, ms, vs), group["lr"], beta1, beta2, group["eps"], group["weight_decay"],
-                        group["step"], self.adamw_mode, group["bias_correction"], inv_scale, noop_flag,
-                        inv_scale_dev)
+                # the staging copies are new tensors every step: a cached table would pin them
+                tbl = mt.TensorTable(ps, gs, ms, vs) if staged else self._table(ps, gs, ms, vs)
+                mt.adam(tbl, group["lr"], beta1, beta2, group["eps"], group["weight_decay"], group["step"],
+                        self.adamw_mode, group["bias_correction"], inv_scale, noop_flag, inv_scale_dev)
             else:
                 adam_reference_step(ps, gs, ms, vs, group["lr"], beta1, beta2, group["eps"], group["weight_decay"],
                                     group["step"], self.adamw_mode, group["bias_correction"], inv_scale)
+            for p, c in staged:
+                p.data.copy_(c)
         return loss

@@ -58,9 +58,13 @@ class FusedLAMB(torch.optim.Optimizer):
                 vs.append(st["exp_avg_sq"])
             if not ps:
                 continue
+            # the trust ratio applies only with nvlamb or a non-zero weight decay (reference stage 2); otherwise a
+            # group (typically biases and norms, weight_decay=0) steps with the plain learning rate
+            trust = bool(self.use_nvlamb or group["weight_decay"] != 0)
             if native:
                 mt.lamb(mt.TensorTable(ps, gs, ms, vs), group["lr"], b1, b2, group["eps"], group["weight_decay"],
-                        group["step"], self.adam_w_mode, group["bias_correction"], group["grad_averaging"], inv_scale)
+                        group["step"], self.adam_w_mode, group["bias_correction"], group["grad_averaging"], inv_scale,
+                        trust_ratio=trust)
             else:
                 bc1 = 1 - b1 ** group["step"] if group["bias_correction"] else 1.0
                 bc2 = 1 - b2 ** group["step"] if group["bias_correction"] else 1.0
@@ -74,7 +78,9 @@ class FusedLAMB(torch.optim.Optimizer):
                     u = (m / bc1) / ((v / bc2).sqrt() + group["eps"])
                     if self.adam_w_mode:
                         u = u + group["weight_decay"] * pf
-                    pn, un = pf.norm(), u.norm()
-                    ratio = torch.where((pn > 0) & (un > 0), pn / un, torch.ones_like(pn))
+                    ratio = 1.0
+                    if trust:
+                        pn, un = pf.norm(), u.norm()
+                        ratio = torch.where((pn > 0) & (un > 0), pn / un, torch.ones_like(pn))
                     p.copy_(pf - group["lr"] * ratio * u)
         return loss

@@ -61,8 +61,12 @@ class TensorTable:
         self.table = torch.tensor(rows, dtype=torch.int64).to(self.device) if n else None
         self._partial = None
         # NOTE: the table stores raw pointers.  Callers own the tensors' lifetime (kernels are stream-ordered, so a
-        # tensor may be released right after the launch); `keepalive=True` pins them for cached tables.
-        self._keepalive = (list(p), g, m, v, lp) if keepalive else None
+        # tensor may be released right after the launch).  `keepalive=True` pins the persistent slots (p, m, v, lp)
+        # for cached tables.  The grad slot is never pinned: gradients are usually new tensors every step, and
+        # pinning them would keep each step's gradients resident and push the next ones to new addresses, so the
+        # cache key (which includes the grad pointers) would never hit.  A key hit means the live gradients sit at
+        # exactly the pointers stored in the table.
+        self._keepalive = (list(p), m, v, lp) if keepalive else None
 
     @staticmethod
     def key_of(*lists) -> tuple:
@@ -133,7 +137,10 @@ def scale(tbl: TensorTable, factor: float, flag: Optional[torch.Tensor] = None) 
 
 def lamb(tbl: TensorTable, lr: float, beta1: float, beta2: float, eps: float, weight_decay: float, step: int,
          adamw: bool = True, bias_correction: bool = True, grad_averaging: bool = True, inv_scale: float = 1.0,
-         noop_flag: Optional[torch.Tensor] = None) -> None:
+         noop_flag: Optional[torch.Tensor] = None, trust_ratio: bool = True) -> None:
+    """Two-stage LAMB.  Stage 1 writes the update u into the grad slot, rounded to the grad dtype; stage 2 steps
+    p -= lr * ratio * u with ratio = ||p|| / ||u|| per tensor (1 if either norm is 0).  `trust_ratio=False` skips
+    both norm launches and steps with ratio 1 (the reference does so unless `use_nvlamb` or weight_decay != 0)."""
     if tbl.num_tensors == 0:
         return
     lib = _get_lib()
@@ -141,12 +148,15 @@ def lamb(tbl: TensorTable, lr: float, beta1: float, beta2: float, eps: float, we
     bc1 = 1.0 - beta1 ** step if bias_correction else 1.0
     bc2 = 1.0 - beta2 ** step if bias_correction else 1.0
     beta3 = 1.0 - beta1 if grad_averaging else 1.0
-    _, p_norms = norm_sq(tbl, "param", per_tensor=True)
+    p_norms = u_norms = None
+    if trust_ratio:
+        _, p_norms = norm_sq(tbl, "param", per_tensor=True)
     loader.check(lib.cb_multi_tensor_lamb_stage1(loader.ptr(tbl.table), tbl.num_tensors,
                                                  ctypes.c_int64(tbl.total_chunks), f(beta1), f(beta2), f(beta3),
                                                  f(eps), f(weight_decay), f(bc1), f(bc2), f(inv_scale), int(adamw),
                                                  loader.ptr(noop_flag), loader.stream_ptr()), "lamb_stage1")
-    _, u_norms = norm_sq(tbl, "grad", per_tensor=True)
+    if trust_ratio:
+        _, u_norms = norm_sq(tbl, "grad", per_tensor=True)
     loader.check(lib.cb_multi_tensor_lamb_stage2(loader.ptr(tbl.table), tbl.num_tensors,
                                                  ctypes.c_int64(tbl.total_chunks), f(lr), loader.ptr(p_norms),
                                                  loader.ptr(u_norms), loader.ptr(noop_flag), loader.stream_ptr()),
