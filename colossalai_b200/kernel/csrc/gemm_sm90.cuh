@@ -294,6 +294,15 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Prob& prob, const
   return (int)cudaGetLastError();
 }
 
+// Host: can store_acc write this output?  out_dtype must be one it knows (any other code would be stored as fp16), and
+// since two adjacent columns go out as one 2-element store (float2 / __nv_bfloat162 / __half2), C's base must be
+// aligned to two elements and ldc must be even (and at least the row width n).
+inline bool epilogue_ok(const void* C, long long ldc, long long n, int out_dtype) {
+  if (out_dtype != CB_F32 && out_dtype != CB_F16 && out_dtype != CB_BF16) return false;
+  const uintptr_t pair_bytes = out_dtype == CB_F32 ? 8 : 4;
+  return ldc >= n && (ldc & 1) == 0 && reinterpret_cast<uintptr_t>(C) % pair_bytes == 0;
+}
+
 // Runtime (a_mn, b_mn, kind) -> template instantiation for 16-bit operands.
 template <class Prob>
 int launch16(const CUtensorMap& ta, const CUtensorMap& tb, const Prob& prob, const Epilogue& e, int grid, bool bf16,

@@ -37,15 +37,18 @@ extern "C" {
 // D[M,N] (+)= A x B^T-like contraction over K.
 //   a_mn_major == 0: A is [M, K] row-major with leading dimension lda;  == 1: A is stored [K, M] (lda between K rows)
 //   b_mn_major == 0: B is [N, K] row-major with leading dimension ldb;  == 1: B is stored [K, N]
-// Requirements: 16-byte aligned base pointers, leading dimensions multiples of 8 elements, ldc multiple of 8 (4 for
-// fp32 output).  M, N, K are otherwise arbitrary (TMA zero-fills out-of-bounds, stores are predicated).  `block_n` is
-// accepted for interface stability; the tile is always 128 x 128.
+// Requirements: 16-byte aligned A / B bases, lda / ldb multiples of 8 elements, K >= 1; out_dtype fp32 / fp16 / bf16,
+// C aligned to two output elements, ldc even and >= N.  M, N, K are otherwise arbitrary (TMA zero-fills out-of-bounds,
+// stores are predicated).  Anything else returns cudaErrorInvalidValue before any work.  `block_n` is accepted for
+// interface stability; the tile is always 128 x 128.
 int cb_gemm_tcgen05(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                     int a_mn_major, int b_mn_major, int in_dtype, int out_dtype, int accumulate, int block_n,
                     cudaStream_t stream) {
   (void)block_n;
-  if (M <= 0 || N <= 0) return 0;
   if (in_dtype != CB_BF16 && in_dtype != CB_F16) return (int)cudaErrorInvalidValue;
+  // K == 0 would need tensor maps of an empty operand, which the driver refuses
+  if (K <= 0 || !epilogue_ok(C, ldc, N, out_dtype)) return (int)cudaErrorInvalidValue;
+  if (M <= 0 || N <= 0) return 0;
   const bool bf16 = in_dtype == CB_BF16;
   CUtensorMap ta, tb;
   int r = tmap16(&ta, A, a_mn_major, M, K, lda, bf16);
@@ -53,19 +56,19 @@ int cb_gemm_tcgen05(const void* A, const void* B, void* C, int M, int N, int K, 
   r = tmap16(&tb, B, b_mn_major, N, K, ldb, bf16);
   if (r) return 2000 + r;
   const DenseProb p = dense(M, N, K, 64);
-  // K == 0: no k-block, the tile stores zeros (or leaves C unchanged when accumulating)
   const Epilogue e{C, ldc, out_dtype, accumulate, nullptr, nullptr};
   return launch16(ta, tb, p, e, grid_for(p), bf16, a_mn_major, b_mn_major, stream);
 }
 
 // D[M,N] (+)= scale_a * scale_b * (A[M,K] x B[N,K]^T) with 8-bit float operands (wgmma m64n128k32, 128 K-elements per
-// stage).  a_fmt / b_fmt: 0 = E4M3, 1 = E5M2.  Requirements: 16-byte aligned bases, lda / ldb multiples of 16 bytes.
-// scale pointers are device fp32 scalars or null.
+// stage).  a_fmt / b_fmt: 0 = E4M3, 1 = E5M2.  Requirements: 16-byte aligned bases, lda / ldb multiples of 16 bytes,
+// K >= 1, and the output rules of cb_gemm_tcgen05.  scale pointers are device fp32 scalars or null.  With accumulate,
+// D = scale_a * scale_b * (A x B^T) + C: the scales apply to the product only.
 int cb_gemm_fp8_tcgen05(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                         int a_fmt, int b_fmt, int out_dtype, int accumulate, const float* scale_a,
                         const float* scale_b, cudaStream_t stream) {
+  if ((lda & 15) || (ldb & 15) || K <= 0 || !epilogue_ok(C, ldc, N, out_dtype)) return (int)cudaErrorInvalidValue;
   if (M <= 0 || N <= 0) return 0;
-  if ((lda & 15) || (ldb & 15)) return (int)cudaErrorInvalidValue;
   CUtensorMap ta, tb;
   int r = make_tmap_2d_8b(&ta, A, M, K, lda, 128, 128);
   if (r) return 1000 + r;

@@ -150,14 +150,17 @@ extern "C" {
 
 // Variable-M grouped GEMM.  x [total_rows, K] (rows grouped by expert, `offs` = cumulative row ends on the device);
 // transpose_b != 0: w [E, N, K] and y = x w[e]^T (forward);  transpose_b == 0: w [E, K, N] and y = x w[e] (dgrad with
-// the forward weight [E, K(out), N(in)]).  y [total_rows, N].  Requirements: contiguous w, K % 8 == 0, N % 8 == 0,
-// 16-byte aligned pointers, E <= 512; transpose_b == 0 additionally needs K % 128 == 0 (a k-block must not straddle
-// two experts' weights).
+// the forward weight [E, K(out), N(in)]).  y [total_rows, N].  Requirements: contiguous w, K % 8 == 0, K >= 8,
+// N % 8 == 0, 16-byte aligned x / w, y aligned to 4 bytes with ldy even and >= N, E <= 512; transpose_b == 0
+// additionally needs K % 128 == 0 (a k-block must not straddle two experts' weights).  Rows after offs[E - 1] are
+// neither read into any group nor written.
 int cb_grouped_gemm(const void* x, const void* w, void* y, const int* offs, int E, int total_rows, int N, int K, int ldx,
                     int ldy, int transpose_b, int dtype, cudaStream_t stream) {
-  if (E <= 0 || total_rows <= 0 || N <= 0) return 0;
-  if (E > MAX_GROUPS || (dtype != CB_BF16 && dtype != CB_F16) || (K & 7) || (N & 7)) return (int)cudaErrorInvalidValue;
+  if (E > MAX_GROUPS || (dtype != CB_BF16 && dtype != CB_F16) || K <= 0 || (K & 7) || (N & 7) ||
+      !epilogue_ok(y, ldy, N, dtype))
+    return (int)cudaErrorInvalidValue;
   if (!transpose_b && (K % 128)) return (int)cudaErrorInvalidValue;
+  if (E <= 0 || total_rows <= 0 || N <= 0) return 0;
   const bool bf16 = dtype == CB_BF16;
   CUtensorMap ta, tb;
   int r = tmap16(&ta, x, false, total_rows, K, ldx, bf16);
@@ -178,11 +181,15 @@ int cb_grouped_gemm(const void* x, const void* w, void* y, const int* offs, int 
 }
 
 // Variable-K grouped GEMM (weight gradients): dw[e] [M, N] (+)= dy[rows of e, M]^T x[rows of e, N].  Every group's row
-// range must start and end on a multiple of 128.  out_dtype: bf16 / fp16 / fp32.
+// range must start and end on a multiple of 128.  out_dtype: bf16 / fp16 / fp32, dw [E, M, N] contiguous and aligned to
+// two output elements, total_rows >= 1 (the operands' tensor maps cannot be empty).  An expert without rows gets
+// dw[e] = 0 (or keeps dw[e] when accumulating).
 int cb_grouped_gemm_wgrad(const void* dy, const void* x, void* dw, const int* offs, int E, int total_rows, int M, int N,
                           int lddy, int ldx, int in_dtype, int out_dtype, int accumulate, cudaStream_t stream) {
+  if (E > MAX_GROUPS || (in_dtype != CB_BF16 && in_dtype != CB_F16) || (M & 7) || (N & 7) || total_rows <= 0 ||
+      !epilogue_ok(dw, N, N, out_dtype))
+    return (int)cudaErrorInvalidValue;
   if (E <= 0 || M <= 0 || N <= 0) return 0;
-  if (E > MAX_GROUPS || (in_dtype != CB_BF16 && in_dtype != CB_F16) || (M & 7) || (N & 7)) return (int)cudaErrorInvalidValue;
   const bool bf16 = in_dtype == CB_BF16;
   CUtensorMap ta, tb;
   int r = tmap16(&ta, dy, true, M, total_rows, lddy, bf16);

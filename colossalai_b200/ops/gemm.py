@@ -70,7 +70,16 @@ def matmul_tn(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = No
     if use_native(a, b):
         n = _try_native()
         if n and n.supported_tn(a, b):
-            return n.gemm_tn(a, b, out=out, accumulate=accumulate)
+            if out is None or n.out_ok(out):
+                return n.gemm_tn(a, b, out=out, accumulate=accumulate)
+            # an output the epilogue cannot store into (a view at an odd element offset, or with an odd row stride):
+            # run the GEMM into a fresh aligned buffer (holding a copy of `out` when accumulating) and write it back
+            if accumulate:
+                o = out.clone(memory_format=torch.contiguous_format)
+            else:
+                o = torch.empty(out.shape, dtype=out.dtype, device=out.device)
+            n.gemm_tn(a, b, out=o, accumulate=accumulate)
+            return out.copy_(o)
     if out is not None and a.is_cuda and out.dtype == a.dtype and out.is_contiguous():
         # library path: accumulate inside the GEMM epilogue (beta = 1) instead of a separate add pass
         if accumulate:

@@ -39,6 +39,20 @@ def _ok2d(t: torch.Tensor) -> bool:
             and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0 and t.stride(0) >= t.shape[1])
 
 
+def out_ok(c: torch.Tensor) -> bool:
+    """True if the epilogue can store into `c`: fp32/bf16/fp16 rows of unit stride, and since two adjacent columns
+    go out as one 2-element store, a base aligned to two elements and an even row stride."""
+    return (c.dim() == 2 and c.dtype in (torch.float32, torch.bfloat16, torch.float16) and c.stride(1) == 1
+            and c.stride(0) % 2 == 0 and c.stride(0) >= c.shape[1] and c.data_ptr() % (2 * c.element_size()) == 0)
+
+
+def _check_out(c: torch.Tensor, M: int, N: int, like: torch.Tensor) -> None:
+    if c.device != like.device or tuple(c.shape) != (M, N) or not out_ok(c):
+        raise ValueError(f"gemm output must be a [{M}, {N}] fp32/bf16/fp16 tensor on {like.device} with unit column "
+                         f"stride, an even row stride and a base aligned to two elements; got {tuple(c.shape)} "
+                         f"{c.dtype} stride {c.stride()} at offset {c.data_ptr() % 16} mod 16 on {c.device}")
+
+
 def _big(m: int, n: int, k: int) -> bool:
     return 2 * m * n * k >= _MIN_FLOPS and k >= 64 and n >= 64
 
@@ -62,6 +76,7 @@ def gemm_nt(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None
     M, K = x.shape
     N = w.shape[0]
     y = out if out is not None else torch.empty(M, N, dtype=x.dtype, device=x.device)
+    _check_out(y, M, N, x)
     _launch(x, w, y, M, N, K, x.stride(0), w.stride(0), 0, 0, False, block_n)
     return y
 
@@ -76,6 +91,7 @@ def gemm_nn(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None
     M, K = a.shape
     N = b.shape[1]
     c = out if out is not None else torch.empty(M, N, dtype=a.dtype, device=a.device)
+    _check_out(c, M, N, a)
     _launch(a, b, c, M, N, K, a.stride(0), b.stride(0), 0, 1, False, block_n)
     return c
 
@@ -93,7 +109,7 @@ def gemm_tn(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None
     if out is None:
         out = torch.empty(M, N, dtype=a.dtype, device=a.device)
         accumulate = False
-    assert out.stride(1) == 1 and out.dtype in (torch.float32, torch.bfloat16, torch.float16)
+    _check_out(out, M, N, a)
     _launch(a, b, out, M, N, red, a.stride(0), b.stride(0), 1, 1, accumulate, block_n)
     return out
 
@@ -133,6 +149,7 @@ def gemm_fp8_nt(a: torch.Tensor, b: torch.Tensor, scale_a: Optional[torch.Tensor
     M, K = a.shape
     N = b.shape[0]
     c = out if out is not None else torch.empty(M, N, dtype=out_dtype, device=a.device)
+    _check_out(c, M, N, a)
     sa = None if scale_a is None else scale_a.reshape(1).to(device=a.device, dtype=torch.float32)
     sb = None if scale_b is None else scale_b.reshape(1).to(device=a.device, dtype=torch.float32)
     lib = _get_lib()

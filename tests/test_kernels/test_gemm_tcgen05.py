@@ -29,51 +29,58 @@ def _tol(K):
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
-@pytest.mark.parametrize("block_n", [128, 256, 512])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("tail", ["none", "half", "ksplit"])
-def test_gemm_nt(M, N, K, block_n, dtype, tail, monkeypatch):
+def test_gemm_nt(M, N, K, dtype):
     from colossalai_b200.ops import gemm_native as g
-
-    _set_tail(monkeypatch, tail)
 
     M = 333 if M == 336 else M     # odd M is fine for K-major A
 
     torch.manual_seed(0)
     x, w = _mk(M, K, dtype=dtype), _mk(N, K, dtype=dtype)
-    y = g.gemm_nt(x, w, block_n=block_n)
+    y = g.gemm_nt(x, w)
     ref = x.float() @ w.float().t()
     torch.testing.assert_close(y.float(), ref, **_tol(K))
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
-@pytest.mark.parametrize("block_n", [128, 256, 512])
-@pytest.mark.parametrize("tail", ["none", "half", "ksplit"])
-def test_gemm_nn(M, N, K, block_n, tail, monkeypatch):
+def test_gemm_nn(M, N, K):
     from colossalai_b200.ops import gemm_native as g
-
-    _set_tail(monkeypatch, tail)
 
     torch.manual_seed(0)
     a, b = _mk(M, K), _mk(K, N)
-    c = g.gemm_nn(a, b, block_n=block_n)
+    c = g.gemm_nn(a, b)
     ref = a.float() @ b.float()
     torch.testing.assert_close(c.float(), ref, **_tol(K))
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
-@pytest.mark.parametrize("block_n", [128, 256, 512])
-@pytest.mark.parametrize("tail", ["none", "half", "ksplit"])
-def test_gemm_tn(M, N, K, block_n, tail, monkeypatch):
+def test_gemm_tn(M, N, K):
     from colossalai_b200.ops import gemm_native as g
-
-    _set_tail(monkeypatch, tail)
 
     torch.manual_seed(0)
     a, b = _mk(K, M), _mk(K, N)      # contraction over dim 0
-    c = g.gemm_tn(a, b, block_n=block_n)
+    c = g.gemm_tn(a, b)
     ref = a.float().t() @ b.float()
     torch.testing.assert_close(c.float(), ref, **_tol(K))
+
+
+def test_gemm_block_n_and_tail_have_no_effect(monkeypatch):
+    """`block_n` and `CB200_GEMM_TAIL_*` are accepted for interface stability and have no effect: every GEMM flavour
+    returns the same bits with and without them."""
+    from colossalai_b200.ops import gemm_native as g
+
+    torch.manual_seed(0)
+    M, N, K = 1000, 768, 520
+    x, w, b, dy = _mk(M, K), _mk(N, K), _mk(K, N), _mk(M, N)
+    base = (g.gemm_nt(x, w), g.gemm_nn(x, b), g.gemm_tn(x, dy))
+    for tail in ("half", "ksplit"):
+        _set_tail(monkeypatch, tail)
+        for block_n in (128, 256, 512):
+            got = (g.gemm_nt(x, w, block_n=block_n), g.gemm_nn(x, b, block_n=block_n),
+                   g.gemm_tn(x, dy, block_n=block_n))
+            for name, r, e in zip(("nt", "nn", "tn"), got, base):
+                assert torch.equal(r.view(torch.int16), e.view(torch.int16)), \
+                    f"gemm_{name} changed with block_n={block_n}, tail={tail}"
 
 
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
