@@ -2,8 +2,8 @@
 save_lora_as_pretrained`, `Booster.enable_lora` booster.py:243-288).
 
 `LoraConfig(r, lora_alpha, target_modules, lora_dropout)`; `apply_lora` freezes the base model and wraps the targeted
-linear layers (plain `nn.Linear` and our TP linears) with a low-rank `B @ A` delta; adapters are saved in the
-peft-compatible layout (`adapter_config.json` + `adapter_model.{bin,safetensors}` with `base_model.model.<name>.lora_A.weight`).
+linear layers (plain `nn.Linear`, our TP linears and the quantised `Linear4bit` / `Linear8bit` of QLoRA) with a
+low-rank `B @ A` delta; adapters are saved in the peft-compatible layout (`adapter_config.json` + `adapter_model.{bin,safetensors}` with `base_model.model.<name>.lora_A.weight`).
 """
 from __future__ import annotations
 
@@ -57,8 +57,12 @@ class LoraLinear(nn.Module):
         self.base_layer = base
         self.r, self.scaling = cfg.r, cfg.lora_alpha / cfg.r
         w = getattr(base, "weight", None)
-        dev = w.device if w is not None else None
-        dt = w.dtype if (w is not None and w.is_floating_point()) else torch.float32
+        if w is None and _is_quantized(base):
+            # a frozen quantised base: adapters in its compute dtype, next to its packed buffers
+            dev, dt = next(base.buffers()).device, base.compute_dtype
+        else:
+            dev = w.device if w is not None else None
+            dt = w.dtype if (w is not None and w.is_floating_point()) else torch.float32
         self.lora_A = nn.Linear(in_features, cfg.r, bias=False, device=dev, dtype=dt)
         self.lora_B = nn.Linear(cfg.r, out_features, bias=False, device=dev, dtype=dt)
         self.lora_dropout = nn.Dropout(cfg.lora_dropout) if cfg.lora_dropout > 0 else nn.Identity()
@@ -85,14 +89,24 @@ class LoraLinear(nn.Module):
         return out + delta.to(out.dtype)
 
     def merge(self) -> None:
+        if _is_quantized(self.base_layer):
+            raise NotImplementedError(
+                f"cannot merge a LoRA adapter into a quantised {type(self.base_layer).__name__}: its weight is packed "
+                "and frozen; load the unquantised base model and merge the saved adapters into it instead")
         if not self.merged and isinstance(self.base_layer, nn.Linear):
             self.base_layer.weight.data += (self.lora_B.weight @ self.lora_A.weight).to(self.base_layer.weight.dtype) \
                 * self.scaling
             self.merged = True
 
 
+def _is_quantized(m: nn.Module) -> bool:
+    from ..quantization.bnb import Linear4bit, Linear8bit
+
+    return isinstance(m, (Linear4bit, Linear8bit))
+
+
 def _linear_dims(m: nn.Module):
-    if isinstance(m, nn.Linear):
+    if isinstance(m, nn.Linear) or _is_quantized(m):
         return m.in_features, m.out_features
     w = getattr(m, "weight", None)
     if w is not None and w.dim() == 2 and hasattr(m, "forward") and type(m).__name__.startswith(("Linear1D", "Linear")):

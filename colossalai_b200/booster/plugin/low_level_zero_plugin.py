@@ -231,4 +231,8 @@ class LowLevelZeroPlugin(DPPluginBase):
         from ..lora import apply_lora
 
         self.lora_enabled = True
+        if bnb_quantization_config is not None:
+            from ...quantization import quantize_model
+
+            model = quantize_model(model, bnb_quantization_config)
         return apply_lora(model, lora_config, pretrained_dir)

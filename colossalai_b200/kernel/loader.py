@@ -50,6 +50,7 @@ LIBS: Dict[str, dict] = {
     "cb200_moe": {"sources": ["moe.cu"], "kind": "cuda"},
     "cb200_infer": {"sources": ["inference.cu"], "kind": "cuda"},
     "cb200_quant": {"sources": ["quant.cu"], "kind": "cuda"},
+    "cb200_wq_gemm": {"sources": ["wq_gemm_wgmma.cu"], "kind": "cuda"},
     "cb200_cpu_adam": {"sources": ["cpu_adam.cpp"], "kind": "cpp"},
     "cb200_aio": {"sources": ["async_file_io.cpp"], "kind": "cpp", "extra": ["-lpthread"]},
 }

@@ -3,7 +3,10 @@
 The reference delegates to bitsandbytes (`colossalai/quantization/bnb.py:30-330`: quantize_model,
 replace_with_bnb_layers, get_keys_to_not_convert, find_tied_parameters).  bitsandbytes is not part of this stack, so the
 quantised layers are implemented here: block-wise absmax scaling, 8-bit signed codes or 4-bit codebook indices packed
-two per byte, dequantise-then-GEMM in the compute dtype (the GEMM itself stays on the bf16 tensor cores).
+two per byte.  On the GPU the forward and the input gradient run on `ops/wq_gemm.py`, whose kernel decodes the packed
+weight inside the GEMM: no 16-bit copy of a frozen weight is kept for backward, which is what lets QLoRA train a model
+whose 16-bit weights would not fit.  The quantisation state (absmax, scales, codebook) stays fp32 whatever dtype the
+module is cast to.
 """
 from __future__ import annotations
 
@@ -18,6 +21,55 @@ from .bnb_config import BnbQuantizationConfig
 __all__ = ["quantize_model", "replace_with_bnb_layers", "get_keys_to_not_convert", "find_tied_parameters",
            "Linear8bit", "Linear4bit"]
 
+# buffers of the quantisation state that must keep full precision through `module.to(dtype)` / `.half()` / `.bfloat16()`
+_FP32_STATE = ("scale", "absmax", "absmax_meta", "code")
+
+
+class _WeightOnlyLinear(torch.autograd.Function):
+    """y = x W^T on a frozen quantised weight.  Only the module (whose buffers are the packed weight) is kept for
+    backward; dX = dY W decodes the weight again."""
+
+    @staticmethod
+    def forward(ctx, x: torch.Tensor, layer: nn.Module) -> torch.Tensor:
+        from ..ops.wq_gemm import wq_linear
+
+        ctx.layer = layer
+        return wq_linear(x, layer)
+
+    @staticmethod
+    def backward(ctx, dy: torch.Tensor):
+        from ..ops.wq_gemm import wq_matmul_nn
+
+        if not ctx.needs_input_grad[0]:
+            return None, None
+        return wq_matmul_nn(dy.contiguous(), ctx.layer), None
+
+
+class _QuantLinearBase(nn.Module):
+    def _apply(self, fn, recurse=True):
+        # a floating-point cast of the module must not round the quantisation state: where `fn` changed a state
+        # buffer's dtype, keep the fp32 original on the device `fn` moved it to
+        state = {n: self._buffers[n] for n in _FP32_STATE if self._buffers.get(n) is not None}
+        super()._apply(fn, recurse)
+        for name, orig in state.items():
+            moved = self._buffers[name]
+            if moved.dtype != orig.dtype:
+                self._buffers[name] = orig.to(device=moved.device)
+        return self
+
+    def dequantize(self) -> torch.Tensor:
+        """The weight in the compute dtype; on the GPU through the native decode kernel, bitwise equal to
+        `dequantize_reference()`."""
+        from ..ops.wq_gemm import dequantize
+
+        return dequantize(self)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        y = _WeightOnlyLinear.apply(x.to(self.compute_dtype), self)
+        if self.bias is not None:
+            y = y + self.bias
+        return y.to(x.dtype)
+
 _NF4 = [-1.0, -0.6961928009986877, -0.5250730514526367, -0.39491748809814453, -0.28444138169288635,
         -0.18477343022823334, -0.09105003625154495, 0.0, 0.07958029955625534, 0.16093020141124725,
         0.24611230194568634, 0.33791524171829224, 0.44070982933044434, 0.5626170039176941, 0.7229568362236023, 1.0]
@@ -25,7 +77,7 @@ _FP4 = [0.0, 0.0052083333, 0.6666667, 1.0, 0.3333333, 0.5, 0.1666667, 0.25,
         -0.0, -0.0052083333, -0.6666667, -1.0, -0.3333333, -0.5, -0.1666667, -0.25]
 
 
-class Linear8bit(nn.Module):
+class Linear8bit(_QuantLinearBase):
     """Row-wise absmax int8 weights."""
 
     def __init__(self, linear: nn.Linear, compute_dtype: torch.dtype) -> None:
@@ -37,14 +89,11 @@ class Linear8bit(nn.Module):
         self.bias = None if linear.bias is None else nn.Parameter(linear.bias.data.to(compute_dtype), False)
         self.in_features, self.out_features, self.compute_dtype = linear.in_features, linear.out_features, compute_dtype
 
-    def dequantize(self) -> torch.Tensor:
+    def dequantize_reference(self) -> torch.Tensor:
         return (self.weight_q.float() * self.scale).to(self.compute_dtype)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        return F.linear(x.to(self.compute_dtype), self.dequantize(), self.bias).to(x.dtype)
 
-
-class Linear4bit(nn.Module):
+class Linear4bit(_QuantLinearBase):
     """Block-wise absmax + 16-entry codebook (nf4 / fp4); optional double quantisation of the absmax vector."""
 
     def __init__(self, linear: nn.Linear, compute_dtype: torch.dtype, quant_type: str = "nf4", block_size: int = 64,
@@ -74,14 +123,11 @@ class Linear4bit(nn.Module):
         self.bias = None if linear.bias is None else nn.Parameter(linear.bias.data.to(compute_dtype), False)
         self.in_features, self.out_features, self.compute_dtype = linear.in_features, linear.out_features, compute_dtype
 
-    def dequantize(self) -> torch.Tensor:
+    def dequantize_reference(self) -> torch.Tensor:
         idx = torch.stack([self.packed >> 4, self.packed & 0xF], dim=1).view(-1).long()
         absmax = (self.absmax_q.float() * self.absmax_meta[1] + self.absmax_meta[0]) if self.double_quant else self.absmax
         w = self.code[idx].view(-1, self.block_size) * absmax[:, None]
         return w.view(-1)[: self.numel].view(self.shape).to(self.compute_dtype)
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        return F.linear(x.to(self.compute_dtype), self.dequantize(), self.bias).to(x.dtype)
 
 
 def find_tied_parameters(model: nn.Module) -> List[List[str]]:
