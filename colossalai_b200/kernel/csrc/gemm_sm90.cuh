@@ -1,10 +1,12 @@
 // Warp-specialised wgmma GEMM main loop for sm_90a, shared by the dense (gemm_wgmma.cu), grouped (grouped_gemm_wgmma.cu)
-// and comm-fused (fused_comm_gemm.cu) GEMMs:  D[128 x 128 tile] (+)= sum_k A(m, k) * B(n, k), fp32 accumulate.
+// and comm-fused (fused_comm_gemm.cu) GEMMs:  D[128 x 128 tile] (+)= sum_k A(m, k) * B(n, k), fp32 accumulate (int32 for
+// the int8 W8A8 GEMM).
 //
 //   * operands are staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) through a STAGES-deep mbarrier ring by one
 //     producer warp (warp 8);
 //   * two consumer warpgroups (warps 0..7) each own 64 rows of the tile and issue wgmma m64n128k16 (16-bit operands) or
-//     m64n128k32 (8-bit float operands) straight from shared memory; the accumulator lives in registers (64 / thread);
+//     m64n128k32 (8-bit float or int8 operands) straight from shared memory; the accumulator lives in registers
+//     (64 / thread);
 //   * a stage is handed back to the producer as soon as the wgmma group reading it has retired (one group in flight);
 //   * A and B may each be K-major ("row = M/N, contiguous K") or MN-major ("row = K, contiguous M/N", 16-bit only),
 //     which covers the three GEMMs of a linear layer without any transposition pass;
@@ -15,6 +17,8 @@
 #pragma once
 #include "common.cuh"
 #include "sm90.cuh"
+
+#include <type_traits>
 
 namespace gemm90 {
 using namespace sm90;
@@ -33,11 +37,14 @@ constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barrier
 constexpr int GROUP_M = 8;
 
 // element kinds of the operands
-enum { K_BF16 = 0, K_F16 = 1, K_E4M3_E4M3 = 2, K_E4M3_E5M2 = 3, K_E5M2_E4M3 = 4, K_E5M2_E5M2 = 5 };
+enum { K_BF16 = 0, K_F16 = 1, K_E4M3_E4M3 = 2, K_E4M3_E5M2 = 3, K_E5M2_E4M3 = 4, K_E5M2_E5M2 = 5, K_S8 = 6 };
 template <int KIND> struct KindTraits {
-  static constexpr bool F8 = KIND >= K_E4M3_E4M3;
-  static constexpr int KE = F8 ? 128 : 64;    // K elements per stage
-  static constexpr int MMA_K = F8 ? 32 : 16;  // K elements per instruction (32 bytes either way)
+  static constexpr bool F8 = KIND >= K_E4M3_E4M3 && KIND <= K_E5M2_E5M2;
+  static constexpr bool S8 = KIND == K_S8;
+  static constexpr int KE = F8 || S8 ? 128 : 64;    // K elements per stage
+  static constexpr int MMA_K = F8 || S8 ? 32 : 16;  // K elements per instruction (32 bytes either way)
+  // int8 products are summed exactly in int32 (|acc| <= 127 * 127 * K: the launcher bounds K)
+  using Acc = typename std::conditional<S8, int, float>::type;
 };
 
 // One tile of work: operand coordinates (elements) and the output window.
@@ -67,6 +74,18 @@ struct Epilogue {
   int accumulate;         // D += existing C
   const float* scale_a;   // fp8 dequantisation: device fp32 scalars multiplied into the product (null = 1)
   const float* scale_b;
+  // int8 (W8A8) output: C = (float(acc) * row_scale[m]) * col_scale[n] + bias[n], each step rounded once
+  const float* row_scale = nullptr;   // fp32 [M] per token, or one device scalar when row_scale_step == 0
+  int row_scale_step = 0;
+  const float* col_scale = nullptr;   // fp32 [N] per output channel
+  const void* bias = nullptr;         // [N] in bias_dtype, or null
+  int bias_dtype = CB_F32;
+  // split-K (W8A8): the K range of an output tile is spread over `splits` CTAs that add their int32 partials into
+  // split_acc [M, N] (ld N) and count arrivals per (tile, warpgroup) in split_cnt; both are zeroed by the caller.  The
+  // last warpgroup to arrive runs the epilogue on the full sum.  Null = each CTA owns the whole K range of its tiles.
+  int* split_acc = nullptr;
+  unsigned* split_cnt = nullptr;
+  int splits = 1;
 };
 
 template <typename T> SM90_DEVICE void store_pair(T* dst, float a, float b, bool two, bool acc) {
@@ -107,9 +126,90 @@ SM90_DEVICE void store_acc(const float (&acc)[64], const Tile& t, const Epilogue
   }
 }
 
+SM90_DEVICE void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+SM90_DEVICE float bias_f32(const void* bias, int dtype, int col) {
+  if (dtype == CB_BF16) return __bfloat162float(static_cast<const __nv_bfloat16*>(bias)[col]);
+  if (dtype == CB_F16) return __half2float(static_cast<const __half*>(bias)[col]);
+  return static_cast<const float*>(bias)[col];
+}
+
+// W8A8 epilogue of one element: the int32 sum converted, scaled per row then per column, biased; explicit roundings so
+// that --use_fast_math contracts nothing (the result is bitwise that of the unfused PyTorch ops).
+SM90_DEVICE float w8a8_value(int acc, const Epilogue& e, int row, int col) {
+  float v = __fmul_rn(__int2float_rn(acc), __ldg(e.row_scale + (size_t)row * e.row_scale_step));
+  v = __fmul_rn(v, __ldg(e.col_scale + col));
+  return e.bias ? __fadd_rn(v, bias_f32(e.bias, e.bias_dtype, col)) : v;
+}
+
+// Store this thread's part of a warpgroup's 64 x 128 int32 accumulator through the W8A8 epilogue.  `flag` is a shared
+// int of this warpgroup (split-K: tells its threads whether this CTA arrived last).
+SM90_DEVICE void store_acc_w8a8(int (&acc)[64], const Tile& t, const Epilogue& e, int wg, int* flag) {
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+  const int r_base = t.row0 + wg * 64 + warp * 16 + (lane >> 2);
+  const int N = t.col_lim;
+  if (e.split_acc) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r_base + 8 * h;
+      if (row >= t.row_lim) continue;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = t.col0 + 8 * j + 2 * (lane & 3);
+        int* dst = e.split_acc + (size_t)row * N + col;
+        if (col < N) atomicAdd(dst, acc[4 * j + 2 * h]);
+        if (col + 1 < N) atomicAdd(dst + 1, acc[4 * j + 2 * h + 1]);
+      }
+    }
+    __threadfence();
+    named_barrier_sync(1 + wg, 128);
+    if ((threadIdx.x & 127) == 0) {
+      const int tile = (t.row0 / BM) * ((N + BN - 1) / BN) + t.col0 / BN;
+      *flag = atomicAdd(e.split_cnt + 2 * tile + wg, 1u) == (unsigned)(e.splits - 1);
+    }
+    named_barrier_sync(1 + wg, 128);
+    if (!*flag) return;
+    __threadfence();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r_base + 8 * h;
+      if (row >= t.row_lim) continue;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = t.col0 + 8 * j + 2 * (lane & 3);
+        const int* src = e.split_acc + (size_t)row * N + col;
+        if (col < N) acc[4 * j + 2 * h] = __ldcg(src);
+        if (col + 1 < N) acc[4 * j + 2 * h + 1] = __ldcg(src + 1);
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = r_base + 8 * h;
+    if (row >= t.row_lim) continue;
+    const size_t roff = (size_t)row * e.ldc;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = t.col0 + 8 * j + 2 * (lane & 3);
+      if (col >= N) continue;
+      const bool two = col + 1 < N;
+      const float a = w8a8_value(acc[4 * j + 2 * h], e, row, col);
+      const float b = two ? w8a8_value(acc[4 * j + 2 * h + 1], e, row, col + 1) : 0.f;
+      if (e.out_dtype == CB_BF16)
+        store_pair((__nv_bfloat16*)e.C + roff + col, a, b, two, false);
+      else if (e.out_dtype == CB_F32)
+        store_pair((float*)e.C + roff + col, a, b, two, false);
+      else
+        store_pair((__half*)e.C + roff + col, a, b, two, false);
+    }
+  }
+}
+
 // The wgmmas of one stage for one consumer warpgroup (rows 64 * wg of A).
-template <int KIND, int A_MN, int B_MN>
-SM90_DEVICE void mma_stage(float (&acc)[64], uint32_t sa, uint32_t sb, int wg) {
+template <int KIND, int A_MN, int B_MN, typename Acc>
+SM90_DEVICE void mma_stage(Acc (&acc)[64], uint32_t sa, uint32_t sb, int wg) {
   using KT = KindTraits<KIND>;
   // A: K-major rows 64 wg .. 64 wg + 63 start 64 rows x 128 B = 8 KB in; MN-major column chunk wg is 8 KB in as well
   const uint64_t da = make_smem_desc_sw128(sa + wg * 8192, A_MN ? 8192 : 16, 1024);
@@ -124,7 +224,8 @@ SM90_DEVICE void mma_stage(float (&acc)[64], uint32_t sa, uint32_t sb, int wg) {
     else if constexpr (KIND == K_E4M3_E4M3) wgmma_ss_m64n128k32_e4m3_e4m3(acc, a, b);
     else if constexpr (KIND == K_E4M3_E5M2) wgmma_ss_m64n128k32_e4m3_e5m2(acc, a, b);
     else if constexpr (KIND == K_E5M2_E4M3) wgmma_ss_m64n128k32_e5m2_e4m3(acc, a, b);
-    else wgmma_ss_m64n128k32_e5m2_e5m2(acc, a, b);
+    else if constexpr (KIND == K_E5M2_E5M2) wgmma_ss_m64n128k32_e5m2_e5m2(acc, a, b);
+    else wgmma_ss_m64n128k32_s8_s8(acc, a, b);
   }
 }
 
@@ -200,9 +301,9 @@ SM90_DEVICE void consumer(const Prob& prob, const Smem& s, const Epilogue& e, in
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const Tile t = prob.tile(tile);
-    float acc[64];
+    typename KindTraits<KIND>::Acc acc[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < 64; ++i) acc[i] = 0;
     int prev = -1;
     for (int kb = 0; kb < t.k_blocks; ++kb) {
       mbar_wait(&s.full[stage], phase);
@@ -233,7 +334,10 @@ SM90_DEVICE void consumer(const Prob& prob, const Smem& s, const Epilogue& e, in
     wgmma_wait<0>();
     reg_fence(acc);
     if (prev >= 0 && leader) mbar_arrive(&s.empty[prev]);
-    store_acc(acc, t, e, wg);
+    if constexpr (KindTraits<KIND>::S8)
+      store_acc_w8a8(acc, t, e, wg, reinterpret_cast<int*>(s.empty + STAGES) + wg);
+    else
+      store_acc(acc, t, e, wg);
     prob.after_store(tile, t, wg);
   }
 }

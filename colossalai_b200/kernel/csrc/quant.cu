@@ -1,4 +1,5 @@
-// FP8 scaled quantisation kernels (per-tensor and per-row scaling) for fp8 communication / fp8 linear.
+// FP8 scaled quantisation kernels (per-tensor and per-row scaling) for fp8 communication / fp8 linear, and the int8
+// per-token (or static-scale) activation quantiser of the SmoothQuant W8A8 linear.
 // Reference behaviour: colossalai/quantization/fp8.py:51-118 (cast_to_fp8 / cast_from_fp8: scale = fp8_max / amax,
 // scale_inv returned to the caller).  Here the amax reduction and the cast are native kernels; the per-row variant is a
 // single pass (row kept in registers between the reduction and the cast).
@@ -62,15 +63,65 @@ __global__ void __launch_bounds__(512) cast_to_fp8_kernel(const T* __restrict__ 
     out[i] = f32_to_fp8<FMT>(to_f32<T>(x[i]) * scale);
 }
 
-// ---- per-row (per-channel) single pass: one CTA per row
+constexpr int FMT_INT8 = 2;
+
+CB_DEVICE uint8_t to_int8(float v, float s) {
+  return (uint8_t)(int8_t)fminf(fmaxf(rintf(__fdiv_rn(v, s)), -127.f), 127.f);
+}
+
+// int8 rows: 16-byte loads when the row allows them (the scalar loop leaves a long decode row latency-bound)
+template <typename T> CB_DEVICE bool vec_row(const T* row, int cols) {
+  return cols % Vec16<T>::N == 0 && reinterpret_cast<uintptr_t>(row) % 16 == 0;
+}
+template <typename T> CB_DEVICE float int8_row_absmax(const T* row, int cols) {
+  constexpr int V = Vec16<T>::N;
+  float m = 0.f;
+  if (vec_row(row, cols)) {
+    for (int c = threadIdx.x * V; c < cols; c += blockDim.x * V) {
+      Vec16<T> v; v.load(row + c);
+#pragma unroll
+      for (int j = 0; j < V; ++j) m = fmaxf(m, fabsf(v.get(j)));
+    }
+  } else {
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) m = fmaxf(m, fabsf(to_f32<T>(row[c])));
+  }
+  return m;
+}
+template <typename T> CB_DEVICE void int8_row_store(const T* row, uint8_t* orow, int cols, float s) {
+  constexpr int V = Vec16<T>::N;
+  if (vec_row(row, cols)) {
+    for (int c = threadIdx.x * V; c < cols; c += blockDim.x * V) {
+      Vec16<T> v; v.load(row + c);
+      uint8_t o[V];
+#pragma unroll
+      for (int j = 0; j < V; ++j) o[j] = to_int8(v.get(j), s);
+      if (V == 8) *reinterpret_cast<uint2*>(orow + c) = *reinterpret_cast<uint2*>(o);
+      else *reinterpret_cast<uint32_t*>(orow + c) = *reinterpret_cast<uint32_t*>(o);
+    }
+  } else {
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) orow[c] = to_int8(to_f32<T>(row[c]), s);
+  }
+}
+
+// ---- per-row (per-channel) single pass: one CTA per row.  FMT 0 / 1: fp8 E4M3 / E5M2 with scale_inv = amax / fp8_max.
+// FMT_INT8: q = clamp(rint(x / s), -127, 127) with s = max(amax, 1e-8) * fl(1 / 127) written to scale_inv (the rounding
+// steps of the PyTorch per-token quantiser on the GPU, which multiplies by the reciprocal of a host scalar divisor), or,
+// with static_scale, s = *static_scale and no reduction (scale_inv is not written).
 template <typename T, int FMT>
 __global__ void __launch_bounds__(256) cast_to_fp8_rows_kernel(const T* __restrict__ x, uint8_t* __restrict__ out,
                                                                int cols, int64_t ld, float* __restrict__ scale_inv,
-                                                               float fp8_max) {
+                                                               float fp8_max, const float* __restrict__ static_scale) {
   const T* row = x + (int64_t)blockIdx.x * ld;
   uint8_t* orow = out + (int64_t)blockIdx.x * cols;
+  if (FMT == FMT_INT8 && static_scale) {
+    int8_row_store(row, orow, cols, __ldg(static_scale));
+    return;
+  }
   float m = 0.f;
-  for (int c = threadIdx.x; c < cols; c += blockDim.x) m = fmaxf(m, fabsf(to_f32<T>(row[c])));
+  if constexpr (FMT == FMT_INT8)
+    m = int8_row_absmax(row, cols);
+  else
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) m = fmaxf(m, fabsf(to_f32<T>(row[c])));
   m = warp_max(m);
   __shared__ float sm[32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -78,10 +129,16 @@ __global__ void __launch_bounds__(256) cast_to_fp8_rows_kernel(const T* __restri
   __syncthreads();
   m = 0.f;
   for (int w = 0; w < (blockDim.x >> 5); ++w) m = fmaxf(m, sm[w]);
-  m = m > 0.f ? m : 1.f;
-  const float scale = fp8_max / m;
-  if (threadIdx.x == 0) scale_inv[blockIdx.x] = m / fp8_max;
-  for (int c = threadIdx.x; c < cols; c += blockDim.x) orow[c] = f32_to_fp8<FMT>(to_f32<T>(row[c]) * scale);
+  if constexpr (FMT == FMT_INT8) {
+    const float s = __fmul_rn(fmaxf(m, 1e-8f), 0x1.020408p-7f);   // fl(1 / 127), not left to fast-math division
+    if (threadIdx.x == 0) scale_inv[blockIdx.x] = s;
+    int8_row_store(row, orow, cols, s);
+  } else {
+    m = m > 0.f ? m : 1.f;
+    const float scale = fp8_max / m;
+    if (threadIdx.x == 0) scale_inv[blockIdx.x] = m / fp8_max;
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) orow[c] = f32_to_fp8<FMT>(to_f32<T>(row[c]) * scale);
+  }
 }
 
 template <typename T, int FMT>
@@ -134,9 +191,24 @@ int cb_fp8_quant_rows(const void* x, void* out, int rows, int cols, int64_t ld, 
   const float fp8_max = fmt == 0 ? 448.f : 57344.f;
   CB_DISPATCH_FLOAT(dtype, T, {
     if (fmt == 0)
-      cast_to_fp8_rows_kernel<T, 0><<<rows, 256, 0, s>>>((const T*)x, (uint8_t*)out, cols, ld, scale_inv, fp8_max);
+      cast_to_fp8_rows_kernel<T, 0><<<rows, 256, 0, s>>>((const T*)x, (uint8_t*)out, cols, ld, scale_inv, fp8_max,
+                                                         nullptr);
     else
-      cast_to_fp8_rows_kernel<T, 1><<<rows, 256, 0, s>>>((const T*)x, (uint8_t*)out, cols, ld, scale_inv, fp8_max);
+      cast_to_fp8_rows_kernel<T, 1><<<rows, 256, 0, s>>>((const T*)x, (uint8_t*)out, cols, ld, scale_inv, fp8_max,
+                                                         nullptr);
+  });
+  return CB_LAUNCH_CHECK();
+}
+
+// W8A8 activations: x [rows, cols] (row stride ld elements, fp32 / fp16 / bf16) -> int8 out [rows, cols] (contiguous).
+// static_scale null: per-row scales to scale[rows] (fp32); else the device fp32 scalar divides every row.
+int cb_int8_quant_rows(const void* x, void* out, int rows, int cols, int64_t ld, float* scale,
+                       const float* static_scale, int dtype, cudaStream_t s) {
+  if (rows < 0 || cols < 0 || ld < cols || (!scale && !static_scale)) return (int)cudaErrorInvalidValue;
+  if (rows == 0 || cols == 0) return 0;
+  CB_DISPATCH_FLOAT(dtype, T, {
+    cast_to_fp8_rows_kernel<T, FMT_INT8><<<rows, 256, 0, s>>>((const T*)x, (uint8_t*)out, cols, ld, scale, 0.f,
+                                                              static_scale);
   });
   return CB_LAUNCH_CHECK();
 }

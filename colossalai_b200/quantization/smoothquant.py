@@ -4,8 +4,10 @@ weights (per output channel) and int8 activations (per token, dynamic) on the in
 
 Parity: reference `colossalai/legacy/inference/quant/smoothquant/models/{base_model.py:1-480, linear.py:1-190,
 llama.py}` (`get_act_scales`, `smooth_ln_fcs`, `W8A8B8O8Linear`, `W8A8BFP32OFP32Linear`, `SmoothLlamaForCausalLM`) —
-those wrap torch-int CUTLASS int8 GEMMs; here the GEMM is `torch._int_mm` (cuBLASLt IMMA) on CUDA with an exact integer
-emulation elsewhere.
+those wrap torch-int CUTLASS int8 GEMMs.  Here, on an sm_90 GPU, `W8A8Linear` runs two native launches per call
+(`ops.w8a8`: the per-token int8 quantiser, then the int8 wgmma GEMM with the scales and bias in its epilogue).  CPU
+tensors and shapes outside that envelope run the PyTorch path below (`torch._int_mm` on CUDA, an exact integer
+emulation on the CPU), which is also the numerics reference.
 """
 from __future__ import annotations
 
@@ -13,6 +15,8 @@ from typing import Dict, Iterable, List, Optional, Sequence
 
 import torch
 import torch.nn as nn
+
+from ..ops import w8a8
 
 __all__ = ["get_act_scales", "smooth_ln_fcs", "quantize_weight_per_channel", "quantize_activation_per_token",
            "W8A8Linear", "smooth_and_quantize_model", "int8_matmul"]
@@ -98,9 +102,26 @@ class W8A8Linear(nn.Module):
             new.bias.data = lin.bias.data.clone().float()
         return new.to(lin.weight.device)
 
+    def _apply(self, fn, recurse=True):
+        # a floating-point cast of the module must not round the quantisation scales: where `fn` changed a scale's
+        # dtype, keep the fp32 original on the device `fn` moved it to
+        state = {n: self._buffers[n] for n in ("weight_scale", "act_scale")}
+        super()._apply(fn, recurse)
+        for name, orig in state.items():
+            moved = self._buffers[name]
+            if moved.dtype != orig.dtype:
+                self._buffers[name] = orig.to(device=moved.device)
+        return self
+
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         shape = x.shape
         x2 = x.reshape(-1, shape[-1])
+        static = None if self.act_quant == "per_token" else self.act_scale
+        # the native GEMM has no backward: a bias that needs a gradient stays on the autograd path below
+        bias_grad = self.bias is not None and self.bias.requires_grad and torch.is_grad_enabled()
+        if not bias_grad and w8a8.supported(x2, self.weight, self.weight_scale, self.bias, static):
+            return w8a8.w8a8_linear(x2, self.weight, self.weight_scale, self.bias, static).reshape(
+                *shape[:-1], self.out_features)
         if self.act_quant == "per_token":
             xq, sx = quantize_activation_per_token(x2)
         else:
