@@ -230,7 +230,7 @@ class BatchBucket:
         if first.output_len == 0 and all(s.output_len == 0 for s in self._sequences_dict.values()):
             out = []
             for s in self._sequences_dict.values():
-                out.extend(s.input_token_id)
+                out.extend(s.input_token_id[s.num_cached_tokens:])       # prefix-cache hits are not recomputed
             return torch.tensor(out, dtype=torch.long, device=self.device)
         if self._use_spec_dec and self._num_tokens_to_verify:
             out = []
@@ -241,6 +241,14 @@ class BatchBucket:
                             dtype=torch.long, device=self.device)
 
     get_1D_inputs_spec_dec = get_1D_inputs
+
+    def block_table_of(self, request_id: int) -> torch.Tensor:
+        """The block-table row of a sequence in this bucket (a view)."""
+        return self._block_tables[self._sequences_indexes[request_id]]
+
+    def get_num_cached_tokens(self) -> List[int]:
+        """Prompt tokens of every sequence (in batch order) whose K/V the prefix cache already holds."""
+        return [s.num_cached_tokens for s in self._sequences_dict.values()]
 
     def get_block_table_tensor(self) -> torch.Tensor:
         return self._block_tables[: self._current_batch_size].to(self.device)

@@ -129,6 +129,9 @@ class InferenceConfig(RPC_PARAM):
     patched_parallelism_size: int = 1
     ignore_eos: bool = False
     use_spec_dec: bool = False
+    # reuse the cached K/V of full blocks whose tokens (and every token before them) equal a prompt's: the prompt's
+    # prefill computes only the rest.  Off by default, like the other cache features.
+    enable_prefix_caching: bool = False
 
     def __post_init__(self) -> None:
         self.max_context_len_to_capture = self.max_input_len + self.max_output_len
@@ -151,6 +154,9 @@ class InferenceConfig(RPC_PARAM):
             assert self.start_token_size <= self.block_size, "start_token_size must fit in one block"
             assert self.generated_token_size % self.block_size == 0
             self.start_token_size = self.block_size
+        # streamingLLM rewrites block tables and rolls blocks out of the window, so blocks cannot be shared
+        assert not (self.enable_prefix_caching and self.enable_streamingllm), \
+            "enable_prefix_caching cannot be combined with enable_streamingllm"
 
     def to_generation_config(self, model_config=None) -> GenerationConfig:
         meta = dict(max_length=self.max_input_len + self.max_output_len, max_new_tokens=self.max_output_len)

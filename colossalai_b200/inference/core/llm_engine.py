@@ -53,6 +53,21 @@ class _SimpleTokenizer:
         return self.batch_decode([ids])[0]
 
 
+def prefix_caching_unsupported(inference_config: InferenceConfig, model_config: ModelConfig) -> Optional[str]:
+    """Why a CUDA engine cannot serve prefix-cache hits natively (None when it can).  A hit runs the prefill through
+    the paged wgmma flash kernel: fp16 / bf16 model and cache, head_dim 64 / 128, no MLA.  Outside that envelope a hit
+    would take the per-sequence reference loop on the GPU."""
+    if inference_config.kv_cache_dtype is not None:
+        return f"the paged prefill kernel reads 16-bit caches, not kv_cache_dtype={inference_config.kv_cache_dtype!r}"
+    if inference_config.dtype not in (torch.float16, torch.bfloat16):
+        return f"the paged prefill kernel needs fp16 or bf16, not {inference_config.dtype}"
+    if getattr(model_config, "use_mla", False):
+        return "MLA models are not supported"
+    if model_config.head_dim not in (64, 128):
+        return f"the paged prefill kernel needs head_dim 64 or 128, not {model_config.head_dim}"
+    return None
+
+
 class LLMEngine(BaseEngine):
     def __init__(self, model_or_path: Union[nn.Module, str, ModelConfig], tokenizer=None,
                  inference_config: Optional[InferenceConfig] = None, verbose: bool = False, model_policy=None) -> None:
@@ -129,6 +144,10 @@ class LLMEngine(BaseEngine):
     def _verify_args(self) -> None:
         assert isinstance(self.inference_config, InferenceConfig), "Invalid type of inference config provided."
         assert isinstance(self.model, nn.Module), f"the model type must be nn.Module, but got {type(self.model)}"
+        if self.inference_config.enable_prefix_caching and torch.device(self.device).type == "cuda":
+            err = prefix_caching_unsupported(self.inference_config, self.model_config)
+            if err:
+                raise ValueError(f"enable_prefix_caching: {err}")
 
     def _init_decode_workspace(self, k_caches, q_per_seq: int = 1) -> None:
         """Size the persistent split-KV buffers of the paged decode kernel for the largest batch (reference
@@ -331,7 +350,11 @@ class LLMEngine(BaseEngine):
         input_ids = batch.get_1D_inputs().to(self.device)
         lens = batch.get_sequence_lengths()
         is_prompt = batch is self.request_handler.prefill_bb
-        positions = self.kv_runtime.set_step(batch.get_block_table_tensor(), lens, is_prompt, self.device)
+        if is_prompt and self.inference_config.enable_prefix_caching:
+            positions = self.kv_runtime.set_step(batch.get_block_table_tensor(), lens, is_prompt, self.device,
+                                                 num_cached=batch.get_num_cached_tokens())
+        else:
+            positions = self.kv_runtime.set_step(batch.get_block_table_tensor(), lens, is_prompt, self.device)
         meta = InputMetaData(block_tables=self.kv_runtime.block_tables, sequence_lengths=self.kv_runtime.seq_lens,
                              batch_size=batch.current_batch_size, is_prompts=is_prompt,
                              use_cuda_kernel=self.inference_config.use_cuda_kernel,

@@ -184,8 +184,13 @@ class RequestHandler(NaiveRequestHandler):
             seqs = self.running_list.prefill[:n]
             if seqs:
                 self.running_list.mark_prefill_running()
-                self.prefill_bb.add_seqs(list(seqs),
-                                         alloc_block_tables_fn=self.cache_manager.allocate_context_from_block_tables)
+                alloc = self.cache_manager.allocate_context_from_block_tables
+                if self.inference_config.enable_prefix_caching:
+                    def alloc(tables, lens, seqs=list(seqs)):
+                        for i, s in enumerate(seqs):
+                            s.num_cached_tokens = self.cache_manager.allocate_context_with_prefix(tables[i],
+                                                                                                  s.input_token_id)
+                self.prefill_bb.add_seqs(list(seqs), alloc_block_tables_fn=alloc)
                 self.running_list.move_prefill_to_decoding([s.request_id for s in seqs])
                 return self.prefill_bb
         # room for this step's token(s) of every running sequence.  The cache is sized for the worst case, so this
@@ -210,6 +215,7 @@ class RequestHandler(NaiveRequestHandler):
 
     def _recycle_last(self) -> None:
         """KV cache exhausted: push the most recent sequence back to the waiting list and free its blocks."""
+        self._index_prefix(self.running_bb, self.running_bb.seqs_li[-1:])
         seqs, _ = self.running_bb.pop_n_seqs(1, self.cache_manager.free_block_table)
         for s in seqs:
             self.running_list.remove(s)
@@ -239,6 +245,8 @@ class RequestHandler(NaiveRequestHandler):
                 if seq in lst:
                     lst.remove(seq)
         else:
+            if request_id in self.running_bb.seqs_ids:
+                self._index_prefix(self.running_bb, [seq])
             self.running_bb.pop_seq_update_batch(request_id, self.cache_manager.free_block_table)
             self.running_list.remove(seq)
         seq.mark_aborted()
@@ -276,7 +284,9 @@ class RequestHandler(NaiveRequestHandler):
     def update(self) -> List[Sequence]:
         """Move freshly prefetched sequences into the decoding bucket, collect finished ones."""
         if not self.prefill_bb.is_empty:
+            self._index_prefix(self.prefill_bb, self.prefill_bb.seqs_li)
             self.running_bb.merge(self.prefill_bb)
+        self._index_prefix(self.running_bb, [s for s in self.running_bb.seqs_li if s.check_finish()])
         finished = self.running_bb.pop_finished(self.cache_manager.free_block_table)
         for s in finished:
             self.running_list.remove(s)
@@ -286,6 +296,15 @@ class RequestHandler(NaiveRequestHandler):
                                                               self.inference_config.generated_token_size)
             self.cache_manager.streamingllm_free_block_tables(freed)
         return finished
+
+    def _index_prefix(self, bucket: BatchBucket, seqs: List[Sequence]) -> None:
+        """Prefix caching: index the full blocks of `seqs` whose K/V are written - every position but the last
+        sampled token's (which has none yet, as have rejected speculative tokens)."""
+        if not self.inference_config.enable_prefix_caching:
+            return
+        for s in seqs:
+            self.cache_manager.register_prefix_blocks(bucket.block_table_of(s.request_id),
+                                                      s.input_token_id + s.output_token_id, s.sentence_len - 1)
 
     def streamingllm_free_block_tables(self, updated_block_ids: List[int]) -> None:
         self.cache_manager.streamingllm_free_block_tables(updated_block_ids)

@@ -55,6 +55,8 @@ class RPCInferenceEngine(LLMEngine):
     def _verify_args(self) -> None:
         assert isinstance(self.inference_config, InferenceConfig)
         assert self.inference_config.pp_size == 1, "RPC engine: tensor parallelism only"
+        if self.inference_config.enable_prefix_caching:
+            raise ValueError("the RPC engine does not support enable_prefix_caching")
 
     # ------------------------------------------------------------------ workers
     def init_workers(self) -> None:

@@ -4,10 +4,18 @@ Parity: reference `colossalai/inference/kv_cache/kvcache_manager.py:18-604`: per
 blocks, free-list allocation for a whole prompt / one decode token / n speculative tokens, block-table maintenance,
 StreamingLLM window eviction, a logical-only RPC variant.
 Layout (H100-first, see kernel/csrc/inference.cu): K and V are both `[num_blocks, block_size, kv_heads, head_dim]`.
+
+Prefix caching (`InferenceConfig.enable_prefix_caching`, no reference equivalent): full blocks whose K/V are written
+are indexed under (serial id of the parent entry, the block's token ids); serial ids are never reused, so an entry
+whose parent was evicted can never match again, even when the parent's block now holds other tokens.  A prompt takes
+references to the longest indexed chain that matches it (at most (L - 1) // block_size blocks: its last token is always
+computed).  Indexed blocks nobody references are *cached-free*: they count as available and are evicted least recently
+freed first, only when no never-indexed free block is left.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Tuple
+from collections import OrderedDict
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -50,6 +58,13 @@ class KVCacheManager:
         self._block_states = torch.ones(self.num_blocks, dtype=torch.bool)
         self._block_states_cum = torch.zeros(self.num_blocks + 1, dtype=torch.int64)
         self._block_finder = torch.zeros(self.num_blocks, dtype=torch.int64)
+        self.enable_prefix_caching = getattr(config, "enable_prefix_caching", False)
+        self._prefix_index: Dict[Tuple[int, Tuple[int, ...]], Tuple[int, int]] = {}   # key -> (block id, serial)
+        self._block_entry: Dict[int, Tuple[Tuple[int, Tuple[int, ...]], int]] = {}    # block id -> (key, serial)
+        self._cached_free: "OrderedDict[int, None]" = OrderedDict()                    # LRU order, oldest first
+        self._next_serial = 1                                                          # 0 = the root
+        self._queried_tokens = 0
+        self._hit_tokens = 0
         if verbose:
             tot = self.total_physical_cache_size_in_bytes / GIGABYTE
             self.logger.info(f"KV cache: {self.num_blocks} blocks x {self.block_size} tokens, {tot:.2f} GB", ranks=[0])
@@ -61,6 +76,11 @@ class KVCacheManager:
     @property
     def num_available_blocks(self) -> int:
         return self._available_blocks
+
+    @property
+    def prefix_cache_stats(self) -> Dict[str, int]:
+        """Prompt tokens looked up in the prefix index and tokens served from it since construction."""
+        return {"queried_tokens": self._queried_tokens, "hit_tokens": self._hit_tokens}
 
     @property
     def total_physical_cache_size_in_bytes(self) -> int:
@@ -86,6 +106,20 @@ class KVCacheManager:
         return k.data_ptr() + off, v.data_ptr() + off
 
     # ------------------------------------------------------------------ allocation
+    def _take_free_blocks(self, n: int) -> List[int]:
+        """`n` blocks for new content: never-indexed free blocks first (lowest ids), then cached-free blocks evicted
+        least recently freed first.  The caller checked that `n` blocks are available."""
+        free = torch.nonzero(self._block_states, as_tuple=False).flatten()[:n].tolist()
+        for bid in free:
+            self._block_states[bid] = False
+        while len(free) < n:
+            bid, _ = self._cached_free.popitem(last=False)
+            key, _ = self._block_entry.pop(bid)
+            del self._prefix_index[key]
+            free.append(bid)
+        self._available_blocks -= n
+        return free
+
     def allocate_context_from_block_table(self, block_table: torch.Tensor, context_len: int) -> None:
         """Allocate the blocks of one prompt; `block_table` is the sequence's 1-D int32 row (-1 = unassigned)."""
         assert block_table.dim() == 1
@@ -94,14 +128,79 @@ class KVCacheManager:
         need = (context_len + self.block_size - 1) // self.block_size
         if need > self._available_blocks:
             raise RuntimeError(f"No enough blocks to allocate. Available {self._available_blocks}; need {need}.")
-        free = torch.nonzero(self._block_states, as_tuple=False).flatten()[:need]
-        block_table[:need] = free.to(block_table.dtype).to(block_table.device)
-        for i, bid in enumerate(free.tolist()):
+        free = self._take_free_blocks(need)
+        block_table[:need] = torch.tensor(free, dtype=block_table.dtype).to(block_table.device)
+        for i, bid in enumerate(free):
             blk = self._cache_blocks[bid]
             blk.add_ref()
             blk.allocate(self.block_size if i < need - 1 else context_len - (need - 1) * self.block_size)
-            self._block_states[bid] = False
-            self._available_blocks -= 1
+
+    def match_prefix(self, token_ids: Sequence[int]) -> List[int]:
+        """Block ids of the longest indexed chain equal to the prompt's leading full blocks, capped at
+        (len - 1) // block_size blocks so that at least one prompt token is computed."""
+        bs = self.block_size
+        parent, hits = 0, []
+        for i in range((len(token_ids) - 1) // bs):
+            entry = self._prefix_index.get((parent, tuple(token_ids[i * bs:(i + 1) * bs])))
+            if entry is None:
+                break
+            hits.append(entry[0])
+            parent = entry[1]
+        return hits
+
+    def allocate_context_with_prefix(self, block_table: torch.Tensor, token_ids: Sequence[int]) -> int:
+        """Allocate one prompt's blocks, sharing the matched prefix chain (`match_prefix`): references are added to
+        the matched blocks (a cached-free block goes from 0 to 1 reference), the rest are fresh.  Returns the number of
+        prompt tokens whose K/V are cached (a whole number of blocks)."""
+        assert block_table.dim() == 1
+        bs, L = self.block_size, len(token_ids)
+        hits = self.match_prefix(token_ids)
+        need = (L + bs - 1) // bs
+        revived = sum(1 for bid in hits if not self._cache_blocks[bid].has_ref())
+        if need - len(hits) > self._available_blocks - revived:
+            raise RuntimeError(f"No enough blocks to allocate. Available {self._available_blocks}; need {need}.")
+        for bid in hits:
+            blk = self._cache_blocks[bid]
+            if not blk.has_ref():
+                del self._cached_free[bid]
+                self._available_blocks -= 1
+                blk.allocate()
+            blk.add_ref()
+        fresh = self._take_free_blocks(need - len(hits))
+        for i, bid in enumerate(fresh):
+            blk = self._cache_blocks[bid]
+            blk.add_ref()
+            pos = (len(hits) + i) * bs
+            blk.allocate(min(bs, L - pos))
+        block_table[:need] = torch.tensor(hits + fresh, dtype=block_table.dtype).to(block_table.device)
+        self._queried_tokens += L
+        self._hit_tokens += len(hits) * bs
+        return len(hits) * bs
+
+    def register_prefix_blocks(self, block_table: torch.Tensor, token_ids: Sequence[int], num_written: int) -> None:
+        """Index the sequence's full blocks whose positions are all `< num_written` (K/V written).  A block whose key
+        is already indexed (the same prefix computed by another sequence) stays out of the index; the chain goes on
+        from the indexed entry."""
+        if not self.enable_prefix_caching:
+            return
+        bs = self.block_size
+        n_full = min(num_written, len(token_ids)) // bs
+        table = block_table[:n_full].tolist()
+        parent = 0
+        for i in range(n_full):
+            bid = table[i]
+            if bid < 0:
+                break
+            key = (parent, tuple(token_ids[i * bs:(i + 1) * bs]))
+            entry = self._prefix_index.get(key)
+            if entry is None:
+                if bid in self._block_entry:          # indexed under another chain: the two chains diverge here
+                    break
+                entry = (bid, self._next_serial)
+                self._next_serial += 1
+                self._prefix_index[key] = entry
+                self._block_entry[bid] = (key, entry[1])
+            parent = entry[1]
 
     def allocate_context_from_block_tables(self, block_tables: torch.Tensor, context_lengths: torch.Tensor) -> None:
         assert block_tables.dim() == 2 and block_tables.size(0) == context_lengths.size(0)
@@ -118,9 +217,7 @@ class KVCacheManager:
         if bid < 0:
             if self._available_blocks < 1:
                 raise RuntimeError("No available blocks to allocate.")
-            bid = int(torch.nonzero(self._block_states, as_tuple=False)[0])
-            self._block_states[bid] = False
-            self._available_blocks -= 1
+            bid = self._take_free_blocks(1)[0]
             self._cache_blocks[bid].add_ref()
             block_table[local] = bid
         self._cache_blocks[bid].allocate(1) if self._cache_blocks[bid].available_space > 0 else None
@@ -144,9 +241,7 @@ class KVCacheManager:
         if bid < 0:
             if self._available_blocks < 1:
                 raise RuntimeError("No available blocks to allocate.")
-            bid = int(torch.nonzero(self._block_states, as_tuple=False)[0])
-            self._block_states[bid] = False
-            self._available_blocks -= 1
+            bid = self._take_free_blocks(1)[0]
             self._cache_blocks[bid].add_ref()
             block_table[block_local_idx] = bid
         return bid
@@ -163,7 +258,10 @@ class KVCacheManager:
             if not blk.has_ref():
                 blk.clear()
                 self._available_blocks += 1
-                self._block_states[bid] = True
+                if bid in self._block_entry:
+                    self._cached_free[bid] = None         # keeps its K/V and index entry until evicted
+                else:
+                    self._block_states[bid] = True
             block_table[i] = -1
 
     def free_block_tables(self, block_tables: torch.Tensor, first_n: Optional[int] = None) -> None:
@@ -176,6 +274,9 @@ class KVCacheManager:
             b.clear()
         self._available_blocks = self.num_blocks
         self._block_states[:] = True
+        self._prefix_index.clear()
+        self._block_entry.clear()
+        self._cached_free.clear()
 
     def streamingllm_free_block_tables(self, updated_block_ids: List[int]) -> None:
         """Free blocks pushed out of the attention window (StreamingLLM)."""

@@ -30,23 +30,30 @@ class PagedKVRuntime:
         self.max_seqlen: int = 0
         self.q_per_seq: int = 1                               # decode: tokens verified per sequence (spec-dec)
         self.max_len_host: int = 0                            # longest sequence of the step (host side, no sync)
+        self.cached_prefix = False                            # prompt step where some sequence hit the prefix cache
 
     def set_step(self, block_tables: torch.Tensor, seq_lens: torch.Tensor, is_prompt: bool, device,
-                 q_per_seq: int = 1) -> torch.Tensor:
-        """Prepare per-step metadata; returns the int64 position of every input token."""
+                 q_per_seq: int = 1, num_cached: Optional[List[int]] = None) -> torch.Tensor:
+        """Prepare per-step metadata; returns the int64 position of every input token.  `num_cached` (prompt steps):
+        per sequence, the leading prompt tokens whose K/V the cache already holds - only positions c_i .. L_i - 1 are
+        fed, and `cu_seqlens` runs over L_i - c_i while `seq_lens` stays L_i."""
         self.block_tables = block_tables.to(device=device, dtype=torch.int32).contiguous()
         self.seq_lens = seq_lens.to(device=device, dtype=torch.int32).contiguous()
         self.is_prompt = is_prompt
         self.q_per_seq = q_per_seq
         lens = seq_lens.tolist()
         self.max_len_host = max(lens) if lens else 0
+        self.cached_prefix = False
         if is_prompt:
-            seq = torch.repeat_interleave(torch.arange(len(lens)), torch.tensor(lens))
-            pos = torch.cat([torch.arange(l) for l in lens])
+            cached = num_cached if num_cached is not None else [0] * len(lens)
+            self.cached_prefix = any(c > 0 for c in cached)
+            new = [l - c for l, c in zip(lens, cached)]
+            seq = torch.repeat_interleave(torch.arange(len(lens)), torch.tensor(new))
+            pos = torch.cat([torch.arange(c, l) for c, l in zip(cached, lens)])
             cu = torch.zeros(len(lens) + 1, dtype=torch.int32)
-            cu[1:] = torch.cumsum(torch.tensor(lens), 0)
+            cu[1:] = torch.cumsum(torch.tensor(new), 0)
             self.cu_seqlens = cu.to(device)
-            self.max_seqlen = max(lens)
+            self.max_seqlen = max(new)
         else:
             seq = torch.repeat_interleave(torch.arange(len(lens)), q_per_seq)
             pos = torch.cat([torch.arange(l - q_per_seq, l) for l in lens])
@@ -59,6 +66,11 @@ class PagedKVRuntime:
                alibi_slopes: Optional[torch.Tensor] = None, sliding_window: Optional[int] = None) -> torch.Tensor:
         kc, vc = self.k_caches[layer_idx], self.v_caches[layer_idx]
         iops.kv_cache_write(k, v, kc, vc, self.block_tables, self.token_seq, self.token_pos)
+        if self.is_prompt and self.cached_prefix:
+            # prefix-cache hit: the new rows attend over the cached prefix and their own K/V, all in the paged cache
+            window = sliding_window if sliding_window is not None and self.max_len_host > sliding_window else None
+            return iops.paged_prefill_attention(q, kc, vc, self.block_tables, self.cu_seqlens, self.seq_lens, scale,
+                                                alibi_slopes=alibi_slopes, window=window)
         if sliding_window is not None and self.max_len_host > sliding_window:
             return self._attend_windowed(q, k, v, kc, vc, scale, alibi_slopes, sliding_window)
         return self._attend_full(q, k, v, kc, vc, scale, alibi_slopes)

@@ -46,6 +46,9 @@ class Sequence:
     def __post_init__(self) -> None:
         self.output_token_id: List[int] = []
         self.status = RequestStatus.WAITING
+        # prompt tokens whose K/V came from the prefix cache at admission (a whole number of blocks); the prefill
+        # computes and writes only the positions from here on
+        self.num_cached_tokens = 0
 
     @property
     def sentence_len(self) -> int:
@@ -86,6 +89,7 @@ class Sequence:
     def recycle(self) -> None:
         assert not self.check_finish() and self.status != RequestStatus.ABORTED
         self.status = RequestStatus.RECYCLED
+        self.num_cached_tokens = 0
 
     def __hash__(self) -> int:
         return hash(self.request_id)

@@ -57,6 +57,13 @@ struct FaParams {
   // EXTRA variant of the kernel only (inference prefill of sliding-window / ALiBi models):
   int window;                        // > 0: query q sees keys (q - window, q]; key tiles left of every window are skipped
   const float* alibi;                // [hq] slopes (score += slope * (key - query)), or null
+  // PAGED variant only (prefill over a paged KV cache): sequence b's cu_seqlens[b + 1] - cu_seqlens[b] new query rows
+  // sit at the absolute positions seq_lens_k[b] - n_b .. seq_lens_k[b] - 1 and see the keys 0 .. seq_lens_k[b] - 1,
+  // read from cache blocks block_tables[b][key / block_size] (k / v tensor maps over [kv_rows, hkv * D])
+  const int* block_tables;           // [batch, max_blocks] int32
+  const int* seq_lens_k;             // [batch] int32: cached + new tokens
+  int block_size, max_blocks;
+  int kv_rows;                       // num_blocks * block_size: a box issued at this row lies past the cache (zeros)
 };
 
 SM90_DEVICE float fast_exp2(float x) {
@@ -114,7 +121,7 @@ SM90_DEVICE void mma_pv(float (&o)[D / 2], const float (&pr)[64], uint32_t sv, b
   }
 }
 
-template <int D, bool EXTRA, bool BF16>
+template <int D, bool EXTRA, bool BF16, bool PAGED>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const FaParams p) {
@@ -133,6 +140,7 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int head = blockIdx.y;
   const int kv_head = head / (p.hq / p.hkv);
   int q_tile, seq_row0, len_q, len_k;
+  int seq = 0;                                 // PAGED: the sequence of this CTA
   if (p.cu_seqlens != nullptr) {
     // packed batch: blockIdx.x enumerates (sequence, query tile) pairs in order; surplus CTAs (the grid is sized for
     // the worst case without knowing the lengths on the host) leave at once
@@ -146,6 +154,7 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     }
     if (bsel < 0) return;                      // uniform across the CTA: no barrier has been touched yet
     q_tile = t; seq_row0 = start; len_q = len; len_k = len;
+    if constexpr (PAGED) { seq = bsel; len_k = p.seq_lens_k[bsel]; }
   } else {
     // heaviest (longest causal) query tiles first
     const int q_tiles = (p.seqlen_q + BLOCK_Q - 1) / BLOCK_Q;
@@ -156,10 +165,14 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int q_row0 = (seq_row0 >= 0 ? seq_row0 : b * p.seqlen_q) + q_tile * BLOCK_Q;   // row in the token-major Q / O
   const int kv_row0 = seq_row0 >= 0 ? seq_row0 : b * p.seqlen_k;
   const int kv_tiles_all = (len_k + BLOCK_KV - 1) / BLOCK_KV;
-  // causal with seqlen_q == seqlen_k: key tiles 0..q_tile; otherwise all of them
-  const int kv_last = p.causal ? min(q_tile + 1, kv_tiles_all) : kv_tiles_all;   // one past the last visible key tile
-  // sliding window: the lowest key any row of this query tile can see is (q_tile * BLOCK_Q - window + 1)
-  const int kv_first = (EXTRA && p.window > 0) ? max(0, q_tile * BLOCK_Q - p.window + 1) / BLOCK_KV : 0;
+  // absolute position of the tile's first query row: PAGED rows follow the sequence's cached tokens (bottom-right
+  // causal diagonal); otherwise queries and keys start together
+  const int q_pos0 = (PAGED ? len_k - len_q : 0) + q_tile * BLOCK_Q;
+  // causal: key tiles up to the one holding the tile's last row (q_tile when seqlen_q == seqlen_k); otherwise all
+  const int kv_last = p.causal ? min(PAGED ? (q_pos0 + BLOCK_Q - 1) / BLOCK_KV + 1 : q_tile + 1, kv_tiles_all)
+                               : kv_tiles_all;                                    // one past the last visible key tile
+  // sliding window: the lowest key any row of this query tile can see is (q_pos0 - window + 1)
+  const int kv_first = (EXTRA && p.window > 0) ? max(0, q_pos0 - p.window + 1) / BLOCK_KV : 0;
   const int kv_tiles = kv_last - kv_first;         // tiles walked; loop index j <-> key tile kv_first + j
   const bool resume = p.o_state != nullptr && p.has_prev != 0;   // block mode: continue from the stored state
 
@@ -190,9 +203,31 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     uint32_t phase = 0;
     for (int j = 0; j < kv_tiles; ++j) {
       mbar_wait(&kv_empty[stage], phase ^ 1);
-      if (lane == 0) {
-        uint8_t* sk = smem_kv + stage * C::KV_STAGE_BYTES;
-        uint8_t* sv = sk + C::K_BYTES;
+      uint8_t* sk = smem_kv + stage * C::KV_STAGE_BYTES;
+      uint8_t* sv = sk + C::K_BYTES;
+      if constexpr (PAGED) {
+        // the 128-key tile is assembled from 128 / block_size boxes of block_size rows, one per lane; every box is a
+        // whole number of 1024-byte swizzle atoms, so the stage has the layout one 128-row box gives.  Boxes of blocks
+        // past the sequence's last one are issued past the end of the cache: TMA fills them with zeros (same byte
+        // count), and their table entries are never read.
+        if (lane == 0) mbar_arrive_expect_tx(&kv_full[stage], C::KV_STAGE_BYTES);
+        __syncwarp();
+        const int bs = p.block_size;
+        if (lane < BLOCK_KV / bs) {
+          const int key = (kv_first + j) * BLOCK_KV + lane * bs;
+          const int kb = key / bs;
+          int row = p.kv_rows;
+          if (key < len_k && kb < p.max_blocks) {
+            const int blk = p.block_tables[(size_t)seq * p.max_blocks + kb];
+            if (blk >= 0) row = blk * bs;
+          }
+#pragma unroll
+          for (int h = 0; h < D / 64; ++h) {
+            tma_load_2d(&tmap_k, &kv_full[stage], sk + h * (BLOCK_KV * 128) + lane * bs * 128, kv_head * D + h * 64, row);
+            tma_load_2d(&tmap_v, &kv_full[stage], sv + h * (BLOCK_KV * 128) + lane * bs * 128, kv_head * D + h * 64, row);
+          }
+        }
+      } else if (lane == 0) {
         mbar_arrive_expect_tx(&kv_full[stage], C::KV_STAGE_BYTES);
         const int row = kv_row0 + (kv_first + j) * BLOCK_KV;
 #pragma unroll
@@ -256,18 +291,21 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     reg_fence(s);
     const int kt = kv_first + j;
     const int k_base = kt * BLOCK_KV;
-    const bool masked = (p.causal && kt == q_tile) || (kt == kv_tiles_all - 1 && (len_k % BLOCK_KV) != 0) ||
-                        (EXTRA && p.window > 0);
+    // PAGED (always causal): a tile is masked when its last key lies after the tile's first query row.  Every query
+    // row sits before the end of its sequence's keys, so that also covers a ragged last tile, and k_lim = q_pos.
+    const bool masked = PAGED ? (k_base + BLOCK_KV - 1 > q_pos0) || (EXTRA && p.window > 0)
+                              : (p.causal && kt == q_tile) || (kt == kv_tiles_all - 1 && (len_k % BLOCK_KV) != 0) ||
+                                    (EXTRA && p.window > 0);
     float mt[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int i = 0; i < 64; ++i) {
       const int h = (i >> 1) & 1;
-      const int q_pos = q_tile * BLOCK_Q + wrow + 8 * h;
+      const int q_pos = q_pos0 + wrow + 8 * h;
       const int key = k_base + 8 * (i >> 2) + cq + (i & 1);
       float x = s[i] * p.scale_log2;
       if (EXTRA) x = fmaf(slope2, (float)(key - q_pos), x);
       if (masked) {
-        const int k_lim = (p.causal && kt == q_tile) ? min(q_pos, len_k - 1) : len_k - 1;
+        const int k_lim = PAGED ? q_pos : (p.causal && kt == q_tile) ? min(q_pos, len_k - 1) : len_k - 1;
         if (key > k_lim || (EXTRA && p.window > 0 && key < q_pos - p.window + 1)) x = -INFINITY;
       }
       s[i] = x;
@@ -336,17 +374,21 @@ template <int D>
 int launch_flash_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int batch, int seqlen_q,
                      int seqlen_k, int hq, int hkv, int causal, float scale, int dtype, cudaStream_t stream,
                      const int* cu_seqlens, long long total_tokens, float* o_state, int has_prev, int window,
-                     const float* alibi) {
+                     const float* alibi, const int* block_tables, const int* seq_lens_k, int block_size,
+                     int max_blocks, int num_blocks) {
   using C = FaCfg<D>;
   const bool bf16 = dtype == CB_BF16;
+  const bool paged = block_tables != nullptr;
   CUtensorMap tq, tk, tv;
   const uint64_t rows_q = cu_seqlens ? (uint64_t)total_tokens : (uint64_t)batch * seqlen_q;
-  const uint64_t rows_k = cu_seqlens ? (uint64_t)total_tokens : (uint64_t)batch * seqlen_k;
+  const uint64_t rows_k = paged ? (uint64_t)num_blocks * block_size
+                                : cu_seqlens ? (uint64_t)total_tokens : (uint64_t)batch * seqlen_k;
+  const uint32_t box_k = paged ? (uint32_t)block_size : BLOCK_KV;
   int r = make_tmap_2d_16b(&tq, q, rows_q, (uint64_t)hq * D, (uint64_t)hq * D, BLOCK_Q, 64, bf16);
   if (r) return 1000 + r;
-  r = make_tmap_2d_16b(&tk, k, rows_k, (uint64_t)hkv * D, (uint64_t)hkv * D, BLOCK_KV, 64, bf16);
+  r = make_tmap_2d_16b(&tk, k, rows_k, (uint64_t)hkv * D, (uint64_t)hkv * D, box_k, 64, bf16);
   if (r) return 2000 + r;
-  r = make_tmap_2d_16b(&tv, v, rows_k, (uint64_t)hkv * D, (uint64_t)hkv * D, BLOCK_KV, 64, bf16);
+  r = make_tmap_2d_16b(&tv, v, rows_k, (uint64_t)hkv * D, (uint64_t)hkv * D, box_k, 64, bf16);
   if (r) return 3000 + r;
   FaParams p;
   p.cu_seqlens = cu_seqlens;
@@ -355,10 +397,15 @@ int launch_flash_fwd(const void* q, const void* k, const void* v, void* out, flo
   p.scale_log2 = scale * LOG2E;
   p.out = out; p.lse = lse; p.out_dtype = dtype;
   p.window = window; p.alibi = alibi;
+  p.block_tables = block_tables; p.seq_lens_k = seq_lens_k; p.block_size = block_size; p.max_blocks = max_blocks;
+  p.kv_rows = paged ? num_blocks * block_size : 0;
   static bool attr_set = false;
   if (!attr_set) {
-    const void* fns[4] = {(const void*)flash_fwd_kernel<D, false, true>, (const void*)flash_fwd_kernel<D, true, true>,
-                          (const void*)flash_fwd_kernel<D, false, false>, (const void*)flash_fwd_kernel<D, true, false>};
+    const void* fns[8] = {
+        (const void*)flash_fwd_kernel<D, false, true, false>, (const void*)flash_fwd_kernel<D, true, true, false>,
+        (const void*)flash_fwd_kernel<D, false, false, false>, (const void*)flash_fwd_kernel<D, true, false, false>,
+        (const void*)flash_fwd_kernel<D, false, true, true>, (const void*)flash_fwd_kernel<D, true, true, true>,
+        (const void*)flash_fwd_kernel<D, false, false, true>, (const void*)flash_fwd_kernel<D, true, false, true>};
     for (const void* f : fns) {
       cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
       if (e != cudaSuccess) return (int)e;
@@ -369,10 +416,15 @@ int launch_flash_fwd(const void* q, const void* k, const void* v, void* out, flo
   dim3 grid(cu_seqlens ? (unsigned)(total_tokens / BLOCK_Q + batch) : (unsigned)((seqlen_q + BLOCK_Q - 1) / BLOCK_Q), hq,
             cu_seqlens ? 1 : batch);
   const bool extra = window > 0 || alibi != nullptr;
-  if (extra && bf16) flash_fwd_kernel<D, true, true><<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
-  else if (bf16) flash_fwd_kernel<D, false, true><<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
-  else if (extra) flash_fwd_kernel<D, true, false><<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
-  else flash_fwd_kernel<D, false, false><<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  decltype(&flash_fwd_kernel<D, false, false, false>) kern;
+  if (paged) {
+    kern = extra ? (bf16 ? flash_fwd_kernel<D, true, true, true> : flash_fwd_kernel<D, true, false, true>)
+                 : (bf16 ? flash_fwd_kernel<D, false, true, true> : flash_fwd_kernel<D, false, false, true>);
+  } else {
+    kern = extra ? (bf16 ? flash_fwd_kernel<D, true, true, false> : flash_fwd_kernel<D, true, false, false>)
+                 : (bf16 ? flash_fwd_kernel<D, false, true, false> : flash_fwd_kernel<D, false, false, false>);
+  }
+  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   return (int)cudaGetLastError();
 }
 
@@ -789,21 +841,35 @@ extern "C" {
 //   prefill : packed and causal with a sliding window (`window` > 0: query q sees keys (q - window, q]; Mistral) and /
 //             or ALiBi slopes (`alibi` [hq] fp32: score += slope * (key - query); BLOOM, Baichuan-13B);
 //   block   : o_state non-null, uniform only (ring attention, see below): the fp32 online-softmax state (o_state
-//             [rows_q, hq, D], lse) is written instead of `out`, and read first when `has_prev`.
+//             [rows_q, hq, D], lse) is written instead of `out`, and read first when `has_prev`;
+//   paged   : block_tables non-null, packed and causal, no o_state (prefill after a prefix-cache hit, and the building
+//             block of chunked prefill): k / v are the paged caches [num_blocks, block_size, hkv, D] (block_size 8, 16,
+//             32, 64 or 128).  Sequence b's new query rows sit at the absolute positions seq_lens_k[b] - n_b ..
+//             seq_lens_k[b] - 1 (n_b from cu_seqlens) and see the keys 0 .. seq_lens_k[b] - 1 through
+//             block_tables[b] (int32 [batch, max_blocks]); window / alibi apply on absolute positions.  seq_lens_k and
+//             block_tables live ON THE DEVICE and are never read by the host; entries past a sequence's last block
+//             are never read (they may be -1 or stale).  lse may be null.
 // Anything outside that envelope returns cudaErrorInvalidValue and launches nothing.
 int cb_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, float* o_state, int has_prev,
                       const int* cu_seqlens, long long total_tokens, int batch, int seqlen_q, int seqlen_k, int hq,
-                      int hkv, int head_dim, int causal, float scale, int window, const float* alibi, int dtype,
-                      cudaStream_t stream) {
+                      int hkv, int head_dim, int causal, float scale, int window, const float* alibi,
+                      const int* block_tables, const int* seq_lens_k, int block_size, int max_blocks, int num_blocks,
+                      int dtype, cudaStream_t stream) {
   const bool packed = cu_seqlens != nullptr;
+  const bool paged = block_tables != nullptr;
+  const bool block_size_ok = block_size == 8 || block_size == 16 || block_size == 32 || block_size == 64 ||
+                             block_size == 128;
   if ((dtype != CB_BF16 && dtype != CB_F16) || hkv <= 0 || hq % hkv || (head_dim != 64 && head_dim != 128) ||
       (!packed && causal && seqlen_q != seqlen_k) || window < 0 || ((window > 0 || alibi) && !(packed && causal)) ||
-      (o_state ? (packed || lse == nullptr) : has_prev != 0))
+      (o_state ? (packed || lse == nullptr) : has_prev != 0) ||
+      (paged ? !(packed && causal && o_state == nullptr && seq_lens_k != nullptr && block_size_ok && max_blocks > 0 &&
+                 num_blocks > 0 && (long long)num_blocks * block_size <= 0x7fffffffLL)
+             : seq_lens_k != nullptr))
     return (int)cudaErrorInvalidValue;
   if (batch <= 0 || (packed ? total_tokens <= 0 : seqlen_q <= 0)) return 0;
   return (head_dim == 128 ? launch_flash_fwd<128> : launch_flash_fwd<64>)(
       q, k, v, out, lse, batch, seqlen_q, seqlen_k, hq, hkv, causal, scale, dtype, stream, cu_seqlens, total_tokens,
-      o_state, has_prev, window, alibi);
+      o_state, has_prev, window, alibi, block_tables, seq_lens_k, block_size, max_blocks, num_blocks);
 }
 
 // Backward of cb_flash_attn_fwd for self attention (seqlen_q == seqlen_k).  q / out / dout / dq [T, hq, D], k / v / dk /

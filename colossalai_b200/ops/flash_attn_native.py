@@ -75,12 +75,15 @@ def _p(addr: int) -> ctypes.c_void_p:
 
 def _fwd(what: str, q: int, k: int, v: int, out: int, lse: int, batch: int, seqlen_q: int, seqlen_k: int, hq: int,
          hkv: int, d: int, causal: bool, scale: float, dtype: torch.dtype, o_state: int = 0, has_prev: bool = False,
-         cu_seqlens: int = 0, total_tokens: int = 0, window: int = 0, alibi: int = 0) -> None:
-    """`cb_flash_attn_fwd` on byte addresses (0 = null); the launcher picks uniform / packed / prefill / block mode."""
+         cu_seqlens: int = 0, total_tokens: int = 0, window: int = 0, alibi: int = 0, block_tables: int = 0,
+         seq_lens: int = 0, block_size: int = 0, max_blocks: int = 0, num_blocks: int = 0) -> None:
+    """`cb_flash_attn_fwd` on byte addresses (0 = null); the launcher picks uniform / packed / prefill / block / paged
+    mode."""
     rc = _get_lib().cb_flash_attn_fwd(_p(q), _p(k), _p(v), _p(out), _p(lse), _p(o_state), int(has_prev),
                                       _p(cu_seqlens), ctypes.c_longlong(total_tokens), batch, seqlen_q, seqlen_k, hq,
-                                      hkv, d, int(causal), ctypes.c_float(scale), int(window), _p(alibi), code(dtype),
-                                      loader.stream_ptr())
+                                      hkv, d, int(causal), ctypes.c_float(scale), int(window), _p(alibi),
+                                      _p(block_tables), _p(seq_lens), int(block_size), int(max_blocks),
+                                      int(num_blocks), code(dtype), loader.stream_ptr())
     loader.check(rc, what)
 
 
@@ -121,6 +124,31 @@ def flash_prefill(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens:
          cu.numel() - 1, 0, 0, Hq, k.shape[1], D, True, scale, q.dtype, cu_seqlens=cu.data_ptr(), total_tokens=T,
          window=window or 0, alibi=slopes.data_ptr() if slopes is not None else 0)
     loader.launch_counter.add("flash_attn_prefill")
+    return out
+
+
+def flash_prefill_paged(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_tables: torch.Tensor,
+                        cu_seqlens_q: torch.Tensor, seq_lens: torch.Tensor, scale: Optional[float], window: int = 0,
+                        alibi_slopes: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Causal prefill of new query rows against keys held in a paged KV cache.  q [T, Hq, D] packs the new rows of
+    every sequence by `cu_seqlens_q` ([B+1]); sequence b's `seq_lens[b]` ([B], cached + new tokens) keys live in the
+    caches [num_blocks, block_size, Hkv, D] (bf16 / fp16, q's dtype) at the blocks `block_tables[b]` ([B, max_blocks]),
+    and its new rows sit at the last n_b of those positions.  `window` / `alibi_slopes` as `flash_prefill`, on absolute
+    positions.  All index tensors stay on the device (no host sync); the table entries past a sequence's last block
+    are never read.  Returns out [T, Hq, D]."""
+    T, Hq, D = q.shape
+    nb, bs, Hkv, _ = k_cache.shape
+    scale = scale if scale is not None else 1.0 / math.sqrt(D)
+    out = torch.empty_like(q)
+    cu = _cu32(cu_seqlens_q, q.device)
+    tables = block_tables.to(device=q.device, dtype=torch.int32).contiguous()
+    lens = seq_lens.to(device=q.device, dtype=torch.int32).contiguous()
+    slopes = alibi_slopes.to(device=q.device, dtype=torch.float32).contiguous() if alibi_slopes is not None else None
+    _fwd("flash_attn_paged_prefill", q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(), 0,
+         cu.numel() - 1, 0, 0, Hq, Hkv, D, True, scale, q.dtype, cu_seqlens=cu.data_ptr(), total_tokens=T,
+         window=window or 0, alibi=slopes.data_ptr() if slopes is not None else 0, block_tables=tables.data_ptr(),
+         seq_lens=lens.data_ptr(), block_size=bs, max_blocks=tables.shape[1], num_blocks=nb)
+    loader.launch_counter.add("flash_attn_paged_prefill")
     return out
 
 

@@ -177,6 +177,57 @@ def paged_decode_attention_ref(q, k_cache, v_cache, block_tables, seq_lens, scal
     return out
 
 
+def paged_prefill_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_tables: torch.Tensor,
+                            cu_seqlens_q: torch.Tensor, seq_lens: torch.Tensor, scale: Optional[float] = None,
+                            alibi_slopes: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
+    """Causal prefill whose keys live in the paged cache: q [T, Hq, D] packs n_b = cu_seqlens_q[b+1] - cu_seqlens_q[b]
+    new rows per sequence; sequence b holds `seq_lens[b]` tokens (cached + new) and its new rows sit at positions
+    seq_lens[b] - n_b .. seq_lens[b] - 1, each attending to every cached position up to its own (the step's K/V must
+    already be written).  `window`: only the last `window` positions a query sees are visible.  fp16 / bf16 queries
+    over a cache of the same dtype at head_dim 64 / 128 run the paged wgmma flash kernel with no host sync; everything
+    else (CPU, fp32, an fp8 cache, other head sizes) takes `paged_prefill_attention_ref`."""
+    D = q.shape[-1]
+    if (use_native(q) and q.dtype in (torch.float16, torch.bfloat16) and k_cache.dtype == q.dtype
+            and v_cache.dtype == q.dtype and D in (64, 128) and q.shape[1] % k_cache.shape[2] == 0):
+        from . import flash_attn_native as fan
+
+        return fan.flash_prefill_paged(q.contiguous(), k_cache, v_cache, block_tables, cu_seqlens_q, seq_lens, scale,
+                                       window=window or 0, alibi_slopes=alibi_slopes)
+    return paged_prefill_attention_ref(q, k_cache, v_cache, block_tables, cu_seqlens_q, seq_lens, scale,
+                                       alibi_slopes, window)
+
+
+def paged_prefill_attention_ref(q, k_cache, v_cache, block_tables, cu_seqlens_q, seq_lens, scale=None,
+                                alibi_slopes=None, window=None):
+    """One sequence at a time: the sequence's K/V gathered from the cache (`gather_paged_kv`, fp8 decoded exactly),
+    then an fp32 masked softmax (float64 for float64 queries)."""
+    T, Hq, D = q.shape
+    Hkv = k_cache.shape[2]
+    scale = scale if scale is not None else 1.0 / math.sqrt(D)
+    G = Hq // Hkv
+    cdt = torch.float64 if q.dtype == torch.float64 else torch.float32
+    out = torch.empty_like(q)
+    cu = cu_seqlens_q.tolist()
+    lens = seq_lens.tolist()
+    for b in range(len(cu) - 1):
+        a, e, L = cu[b], cu[b + 1], lens[b]
+        if e == a:
+            continue
+        k = gather_paged_kv(k_cache, block_tables[b], L, cdt).repeat_interleave(G, dim=1)
+        v = gather_paged_kv(v_cache, block_tables[b], L, cdt).repeat_interleave(G, dim=1)
+        q_pos = torch.arange(L - (e - a), L, device=q.device)
+        rel = torch.arange(L, device=q.device)[None, :] - q_pos[:, None]           # key - query
+        keep = rel <= 0
+        if window is not None and window > 0:
+            keep = keep & (rel > -window)
+        s = torch.einsum("qhd,khd->hqk", q[a:e].to(cdt), k) * scale
+        if alibi_slopes is not None:
+            s = s + alibi_slopes.to(device=q.device, dtype=cdt)[:, None, None] * rel.to(cdt)[None]
+        s = s.masked_fill(~keep[None], float("-inf"))
+        out[a:e] = torch.einsum("hqk,khd->qhd", s.softmax(-1), v).to(q.dtype)
+    return out
+
+
 def convert_fp8(x: torch.Tensor, to_fp8: bool, out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
     """KV-cache fp8 (e5m2) storage conversion."""
     if to_fp8:
