@@ -134,6 +134,7 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   uint64_t* q_full = bars;                 // [1]
   uint64_t* kv_full = bars + 1;            // [2]
   uint64_t* kv_empty = bars + 3;           // [2]  one arrival per consumer warpgroup
+  uint64_t* kv_land = bars + 5;            // [1]  the ragged last key tile, landed but not yet released
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -182,6 +183,7 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       mbar_init(&kv_full[i], 1);
       mbar_init(&kv_empty[i], 2);
     }
+    mbar_init(kv_land, 1);
     fence_barrier_init();
   }
   if (warp == PRODUCER_WARP && lane == 0) {
@@ -199,18 +201,25 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       for (int h = 0; h < D / 64; ++h)                     // boxes [128 rows, 64 d] -> K-major swizzled sub-tiles
         tma_load_2d(&tmap_q, q_full, smem_q + h * (BLOCK_Q * 128), head * D + h * 64, q_row0);
     }
+    const bool ragged = (len_k % BLOCK_KV) != 0 && kv_last == kv_tiles_all;   // the walk ends on a partial key tile
     int stage = 0;
     uint32_t phase = 0;
     for (int j = 0; j < kv_tiles; ++j) {
       mbar_wait(&kv_empty[stage], phase ^ 1);
       uint8_t* sk = smem_kv + stage * C::KV_STAGE_BYTES;
       uint8_t* sv = sk + C::K_BYTES;
+      // The rows of a ragged last key tile past the sequence's keys hold another sequence's rows (the tensor maps span
+      // the whole packed / batched tensor) or a paged block's unwritten tail slots.  Their P is 0, but 0 * NaN or Inf
+      // in the P V MMA is NaN.  So that tile lands on kv_land instead: this warp zeroes those V rows (128-byte rows of
+      // each 64-column sub-tile, whatever the swizzle) and only then releases the stage to the consumers.
+      const bool clean = ragged && j == kv_tiles - 1;
+      uint64_t* full = clean ? kv_land : &kv_full[stage];
       if constexpr (PAGED) {
         // the 128-key tile is assembled from 128 / block_size boxes of block_size rows, one per lane; every box is a
         // whole number of 1024-byte swizzle atoms, so the stage has the layout one 128-row box gives.  Boxes of blocks
         // past the sequence's last one are issued past the end of the cache: TMA fills them with zeros (same byte
         // count), and their table entries are never read.
-        if (lane == 0) mbar_arrive_expect_tx(&kv_full[stage], C::KV_STAGE_BYTES);
+        if (lane == 0) mbar_arrive_expect_tx(full, C::KV_STAGE_BYTES);
         __syncwarp();
         const int bs = p.block_size;
         if (lane < BLOCK_KV / bs) {
@@ -223,20 +232,34 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           }
 #pragma unroll
           for (int h = 0; h < D / 64; ++h) {
-            tma_load_2d(&tmap_k, &kv_full[stage], sk + h * (BLOCK_KV * 128) + lane * bs * 128, kv_head * D + h * 64, row);
-            tma_load_2d(&tmap_v, &kv_full[stage], sv + h * (BLOCK_KV * 128) + lane * bs * 128, kv_head * D + h * 64, row);
+            tma_load_2d(&tmap_k, full, sk + h * (BLOCK_KV * 128) + lane * bs * 128, kv_head * D + h * 64, row);
+            tma_load_2d(&tmap_v, full, sv + h * (BLOCK_KV * 128) + lane * bs * 128, kv_head * D + h * 64, row);
           }
         }
       } else if (lane == 0) {
-        mbar_arrive_expect_tx(&kv_full[stage], C::KV_STAGE_BYTES);
+        mbar_arrive_expect_tx(full, C::KV_STAGE_BYTES);
         const int row = kv_row0 + (kv_first + j) * BLOCK_KV;
 #pragma unroll
         for (int h = 0; h < D / 64; ++h) {
-          tma_load_2d(&tmap_k, &kv_full[stage], sk + h * (BLOCK_KV * 128), kv_head * D + h * 64, row);
-          tma_load_2d(&tmap_v, &kv_full[stage], sv + h * (BLOCK_KV * 128), kv_head * D + h * 64, row);
+          tma_load_2d(&tmap_k, full, sk + h * (BLOCK_KV * 128), kv_head * D + h * 64, row);
+          tma_load_2d(&tmap_v, full, sv + h * (BLOCK_KV * 128), kv_head * D + h * 64, row);
         }
       }
       __syncwarp();
+      if (clean) {
+        mbar_wait(kv_land, 0);
+        const int r0 = len_k - (kv_tiles_all - 1) * BLOCK_KV;
+        const int per_sub = (BLOCK_KV - r0) * 8;                       // 16-byte chunks past row r0 in one sub-tile
+#pragma unroll 1
+        for (int i = lane; i < per_sub * (D / 64); i += 32) {
+          const int h = i / per_sub;
+          *reinterpret_cast<uint4*>(sv + r0 * 128 + h * (BLOCK_KV * 128) + (i - h * per_sub) * 16) =
+              make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async();                                           // generic writes -> the wgmma (async proxy)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&kv_full[stage]);
+      }
       if (++stage == KV_STAGES) { stage = 0; phase ^= 1; }
     }
     return;
@@ -850,6 +873,11 @@ extern "C" {
 //             block_tables live ON THE DEVICE and are never read by the host; entries past a sequence's last block
 //             are never read (they may be -1 or stale).  lse may be null.
 // Anything outside that envelope returns cudaErrorInvalidValue and launches nothing.
+// Sequences do not see each other: the out / lse rows of a sequence (a packed sequence, a batch entry of a uniform
+// call, a paged sequence) depend only on that sequence's q / k / v rows, even where other rows hold NaN or Inf: a
+// ragged last key tile zeroes its V rows past the sequence's keys, and a paged sequence's unwritten tail slots need
+// not be finite.  As in flash-attn 2, keys a causal row must not see INSIDE its own sequence's diagonal tile are masked
+// to p = 0 but still enter the P V MMA, so a NaN / Inf value in a future key of the same sequence reaches earlier rows.
 int cb_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, float* lse, float* o_state, int has_prev,
                       const int* cu_seqlens, long long total_tokens, int batch, int seqlen_q, int seqlen_k, int hq,
                       int hkv, int head_dim, int causal, float scale, int window, const float* alibi,
@@ -875,6 +903,10 @@ int cb_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, fl
 // Backward of cb_flash_attn_fwd for self attention (seqlen_q == seqlen_k).  q / out / dout / dq [T, hq, D], k / v / dk /
 // dv [T, hkv, D], lse [T, hq] fp32 from the forward.  Workspaces: delta [T, hq] fp32 and dq_acc [T, hq, D] fp32 (this
 // function zeroes dq_acc).  dtype and GQA as the forward; head_dim 128.
+// Unlike the forward, the gradients of a sequence are NOT independent of the rows after it: a ragged last key tile or
+// query tile loads the next sequence's (or batch entry's) q / k / dout rows, and although their P and dS are forced to
+// 0, 0 * NaN or Inf in the dV / dK / dQ MMAs is NaN.  Non-finite values in one packed sequence can therefore corrupt
+// the gradients of the sequence before it.
 int cb_flash_attn_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
                       void* dq, void* dk, void* dv, float* delta, float* dq_acc, int batch, int seqlen, int hq, int hkv,
                       int head_dim, int causal, float scale, int dtype, const int* cu_seqlens, long long total_tokens,
