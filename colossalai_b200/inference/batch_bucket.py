@@ -211,11 +211,12 @@ class BatchBucket:
         self._current_batch_size = 0
         return ids
 
-    def merge(self, other: "BatchBucket") -> List[int]:
-        """Move as many sequences of `other` as fit into this bucket (block tables travel with them)."""
+    def merge(self, other: "BatchBucket", request_ids: Optional[List[int]] = None) -> List[int]:
+        """Move as many sequences of `other` (only those in `request_ids` when given) as fit into this bucket (block
+        tables travel with them)."""
         unmerged = []
-        n = min(self.available_batch_size, other.current_batch_size)
-        ids = other.seqs_ids
+        ids = other.seqs_ids if request_ids is None else list(request_ids)
+        n = min(self.available_batch_size, len(ids))
         for rid in ids[:n]:
             seq, table = other.pop_seq_update_batch(rid)
             self.add_seq(seq, alloc_block_table=table)

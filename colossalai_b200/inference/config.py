@@ -132,6 +132,10 @@ class InferenceConfig(RPC_PARAM):
     # reuse the cached K/V of full blocks whose tokens (and every token before them) equal a prompt's: the prompt's
     # prefill computes only the rest.  Off by default, like the other cache features.
     enable_prefix_caching: bool = False
+    # chunked prefill: no step feeds the model more than this many tokens.  Every decoding sequence feeds its token and
+    # prompt chunks fill the rest, so a long prompt no longer stalls the running streams.  None: whole prompts, with
+    # prefill and decode in separate steps.
+    max_num_batched_tokens: Optional[int] = None
 
     def __post_init__(self) -> None:
         self.max_context_len_to_capture = self.max_input_len + self.max_output_len
@@ -157,6 +161,15 @@ class InferenceConfig(RPC_PARAM):
         # streamingLLM rewrites block tables and rolls blocks out of the window, so blocks cannot be shared
         assert not (self.enable_prefix_caching and self.enable_streamingllm), \
             "enable_prefix_caching cannot be combined with enable_streamingllm"
+        if self.max_num_batched_tokens is not None:
+            n = self.max_num_batched_tokens
+            # chunks end on block boundaries, and every step has room for one block of prompt after one token per
+            # running sequence
+            assert n > 0 and n % self.block_size == 0, "max_num_batched_tokens must be a positive multiple of block_size"
+            assert n >= self.max_batch_size + self.block_size, \
+                "max_num_batched_tokens must be at least max_batch_size + block_size"
+            assert not self.enable_streamingllm, "max_num_batched_tokens cannot be combined with enable_streamingllm"
+            assert self.beam_width == 1, "max_num_batched_tokens cannot be combined with beam_width > 1"
 
     def to_generation_config(self, model_config=None) -> GenerationConfig:
         meta = dict(max_length=self.max_input_len + self.max_output_len, max_new_tokens=self.max_output_len)

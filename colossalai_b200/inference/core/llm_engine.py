@@ -6,7 +6,7 @@ Parity: reference `colossalai/inference/core/llm_engine.py:46-758` (`init_model`
 from __future__ import annotations
 
 import time
-from itertools import count
+from itertools import accumulate, count
 from typing import Dict, List, Optional, Tuple, Union
 
 import numpy as np
@@ -148,6 +148,11 @@ class LLMEngine(BaseEngine):
             err = prefix_caching_unsupported(self.inference_config, self.model_config)
             if err:
                 raise ValueError(f"enable_prefix_caching: {err}")
+        if self.inference_config.max_num_batched_tokens is not None and torch.device(self.device).type == "cuda":
+            # every chunk runs the paged prefill, as a prefix-cache hit does
+            err = prefix_caching_unsupported(self.inference_config, self.model_config)
+            if err:
+                raise ValueError(f"max_num_batched_tokens: {err}")
 
     def _init_decode_workspace(self, k_caches, q_per_seq: int = 1) -> None:
         """Size the persistent split-KV buffers of the paged decode kernel for the largest batch (reference
@@ -363,6 +368,8 @@ class LLMEngine(BaseEngine):
         return input_ids, positions, meta
 
     def _step_with_batch(self, batch: BatchBucket) -> List[Sequence]:
+        if self.inference_config.max_num_batched_tokens is not None and batch is self.request_handler.prefill_bb:
+            return self._step_chunked()
         input_ids, positions, meta = self.prepare_input(batch)
         bs = batch.current_batch_size
         if self.use_cuda_graph and not meta.is_prompts and bs in self.graph_runners:
@@ -374,15 +381,45 @@ class LLMEngine(BaseEngine):
         if meta.is_prompts:   # keep the logits of the last prompt token of every sequence
             last = (self.kv_runtime.cu_seqlens[1:] - 1).long()
             logits = logits[last]
+        next_tokens = self._sample(logits, meta.is_prompts, meta.batch_token_ids)
+        self.request_handler.append_next_tokens(next_tokens.cpu())
+        return self.request_handler.update()
+
+    def _sample(self, logits: torch.Tensor, is_prompts: bool, batch_token_ids: List[List[int]]) -> torch.Tensor:
         logits = logits[:, : self.model_config.vocab_size]
         if self.tp_group is not None and logits.shape[-1] < self.model_config.vocab_size:
             from ...parallel import comm
 
             logits = comm.all_gather(logits.contiguous(), -1, self.tp_group)[:, : self.model_config.vocab_size]
-        next_tokens = search_tokens(self.generation_config, logits, meta.is_prompts,
-                                    batch_token_ids=meta.batch_token_ids)
-        self.request_handler.append_next_tokens(next_tokens.cpu())
-        return self.request_handler.update()
+        return search_tokens(self.generation_config, logits, is_prompts, batch_token_ids=batch_token_ids)
+
+    def _step_chunked(self) -> List[Sequence]:
+        """One chunked-prefill step (`RequestHandler._schedule_chunks`): the planned prompt chunks, then one token of
+        every decoding sequence, in one forward.  It samples the last row of every prompt the step completes and every
+        decode row, in one call; a prompt with chunks left samples nothing."""
+        rh = self.request_handler
+        pre, dec = rh.prefill_bb, rh.running_bb
+        n_dec = dec.current_batch_size if rh.decode_in_step else 0
+        seqs = pre.seqs_li[: len(rh.prefill_chunks)]
+        starts = [s.num_cached_tokens for s in seqs]
+        ends = [c + n for c, n in zip(starts, rh.prefill_chunks)]
+        ids = [t for s, c, e in zip(seqs, starts, ends) for t in s.input_token_id[c:e]]
+        if n_dec:
+            ids += dec.get_1D_inputs().tolist()
+        tables = torch.cat([pre.block_tables[: len(seqs)], dec.block_tables[:n_dec]])
+        lens = torch.tensor(ends + dec.seq_lengths[:n_dec].tolist(), dtype=torch.int32)
+        positions = self.kv_runtime.set_chunked_step(tables, lens, starts, self.device)
+        logits = self._model_forward(torch.tensor(ids, dtype=torch.long, device=self.device), positions)
+        cu = list(accumulate(rh.prefill_chunks))
+        done = [i for i, (s, e) in enumerate(zip(seqs, ends)) if e == s.input_len]
+        pick = [cu[i] - 1 for i in done] + list(range(cu[-1], cu[-1] + n_dec))
+        tokens = []
+        if pick:
+            token_ids = [seqs[i].input_token_id for i in done] + (dec.batch_token_ids if n_dec else [])
+            rows = torch.tensor(pick, dtype=torch.long, device=self.device)
+            tokens = self._sample(logits[rows], False, token_ids).tolist()
+        rh.append_chunked_tokens(tokens)
+        return rh.update()
 
     @torch.inference_mode()
     def step(self) -> List[Sequence]:

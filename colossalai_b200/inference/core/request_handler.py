@@ -140,6 +140,9 @@ class RequestHandler(NaiveRequestHandler):
                   generated_token_size=inference_config.generated_token_size)
         self.running_bb = BatchBucket(**kw)
         self.prefill_bb = BatchBucket(**kw)
+        # chunked prefill: the step `_schedule_chunks` planned
+        self.prefill_chunks: List[int] = []
+        self.decode_in_step = False
 
     def _init_cache(self, model_config) -> None:
         self.cache_manager = KVCacheManager(self.inference_config, model_config)
@@ -162,7 +165,8 @@ class RequestHandler(NaiveRequestHandler):
         self.running_bb.reset_use_spec_dec()
 
     def schedule(self) -> BatchBucket:
-        """Returns the bucket to run this step: a prefill bucket when enough prompts are waiting, else decoding."""
+        """Returns the bucket to run this step: a prefill bucket when enough prompts are waiting, else decoding.  With
+        `max_num_batched_tokens` set, see `_schedule_chunks`."""
         if self._has_waiting():
             for lst in reversed(self.waiting_list):
                 if not lst:
@@ -179,20 +183,65 @@ class RequestHandler(NaiveRequestHandler):
                     seq = lst.pop(0)
                     self.running_list.append(seq)
                     remain -= 1
+        if self.inference_config.max_num_batched_tokens is not None:
+            return self._schedule_chunks()
         if self.running_list.ready_for_prefill() and self.prefill_bb.is_empty:
             n = min(self.running_list.prefill_seq_num, self.running_bb.available_batch_size)
             seqs = self.running_list.prefill[:n]
             if seqs:
-                self.running_list.mark_prefill_running()
-                alloc = self.cache_manager.allocate_context_from_block_tables
-                if self.inference_config.enable_prefix_caching:
-                    def alloc(tables, lens, seqs=list(seqs)):
-                        for i, s in enumerate(seqs):
-                            s.num_cached_tokens = self.cache_manager.allocate_context_with_prefix(tables[i],
-                                                                                                  s.input_token_id)
-                self.prefill_bb.add_seqs(list(seqs), alloc_block_tables_fn=alloc)
-                self.running_list.move_prefill_to_decoding([s.request_id for s in seqs])
+                self._start_prefill(seqs)
                 return self.prefill_bb
+        self._reserve_decode_tokens()
+        return self.running_bb
+
+    def _start_prefill(self, seqs: List[Sequence]) -> None:
+        """Move admitted prompts into the prefill bucket with blocks for their whole prompt (sharing prefix-cache
+        hits)."""
+        self.running_list.mark_prefill_running()
+        alloc = self.cache_manager.allocate_context_from_block_tables
+        if self.inference_config.enable_prefix_caching:
+            def alloc(tables, lens, seqs=list(seqs)):
+                for i, s in enumerate(seqs):
+                    s.num_cached_tokens = self.cache_manager.allocate_context_with_prefix(tables[i],
+                                                                                          s.input_token_id)
+        self.prefill_bb.add_seqs(list(seqs), alloc_block_tables_fn=alloc)
+        self.running_list.move_prefill_to_decoding([s.request_id for s in seqs])
+
+    def _schedule_chunks(self) -> BatchBucket:
+        """Chunked prefill.  Admitted prompts join the prefill bucket at once and stay there until their last chunk
+        has run.  A step holds one token of every decoding sequence, then prompt chunks up to `max_num_batched_tokens`
+        in total, first come first served: a prompt gets tokens only once every earlier prompt is fully scheduled.
+        Every chunk but a prompt's last is a whole number of blocks, and chunks start where the cached tokens end, on a
+        block boundary.  Speculative decoding verifies in a pass of its own, so while prompts are pending its steps
+        hold chunks only.
+
+        Returns the prefill bucket when the step feeds chunks - `prefill_chunks[i]` tokens of its i-th sequence,
+        followed by the decoding bucket's rows when `decode_in_step` - else the decoding bucket (a plain decode
+        step)."""
+        seqs = self.running_list.prefill
+        if seqs:
+            self._start_prefill(seqs)
+        budget = self.inference_config.max_num_batched_tokens
+        self.decode_in_step = self.prefill_bb.is_empty or not self.running_bb.use_spec_dec
+        if self.decode_in_step:
+            self._reserve_decode_tokens()
+            budget -= self.running_bb.current_batch_size
+        bs = self.inference_config.block_size
+        self.prefill_chunks = []
+        for s in self.prefill_bb.seqs_li:
+            left = s.input_len - s.num_cached_tokens
+            n = min(left, budget)
+            if n < left:
+                n -= n % bs
+            if n == 0:
+                break
+            self.prefill_chunks.append(n)
+            budget -= n
+            if n < left:
+                break
+        return self.prefill_bb if self.prefill_chunks else self.running_bb
+
+    def _reserve_decode_tokens(self) -> None:
         # room for this step's token(s) of every running sequence.  The cache is sized for the worst case, so this
         # only fails under over-subscription (speculative look-ahead); then the youngest sequence goes back to the
         # waiting list and the allocation is RETRIED - the failed pass stopped at the first sequence without a block,
@@ -211,12 +260,13 @@ class RequestHandler(NaiveRequestHandler):
                 break
             except RuntimeError:
                 self._recycle_last()
-        return self.running_bb
 
     def _recycle_last(self) -> None:
-        """KV cache exhausted: push the most recent sequence back to the waiting list and free its blocks."""
-        self._index_prefix(self.running_bb, self.running_bb.seqs_li[-1:])
-        seqs, _ = self.running_bb.pop_n_seqs(1, self.cache_manager.free_block_table)
+        """KV cache exhausted: push the most recent sequence back to the waiting list and free its blocks.  Prompts
+        still being prefilled (chunked prefill) are younger than every decoding sequence, so they go first."""
+        bucket = self.running_bb if self.prefill_bb.is_empty else self.prefill_bb
+        self._index_prefix(bucket, bucket.seqs_li[-1:])
+        seqs, _ = bucket.pop_n_seqs(1, self.cache_manager.free_block_table)
         for s in seqs:
             self.running_list.remove(s)
             s.recycle()
@@ -245,9 +295,10 @@ class RequestHandler(NaiveRequestHandler):
                 if seq in lst:
                     lst.remove(seq)
         else:
-            if request_id in self.running_bb.seqs_ids:
-                self._index_prefix(self.running_bb, [seq])
-            self.running_bb.pop_seq_update_batch(request_id, self.cache_manager.free_block_table)
+            for bucket in (self.running_bb, self.prefill_bb):      # a prompt mid-prefill sits in the prefill bucket
+                if request_id in bucket.seqs_ids:
+                    self._index_prefix(bucket, [seq])
+                    bucket.pop_seq_update_batch(request_id, self.cache_manager.free_block_table)
             self.running_list.remove(seq)
         seq.mark_aborted()
 
@@ -281,9 +332,25 @@ class RequestHandler(NaiveRequestHandler):
         else:
             self.running_bb.append_batch_tokens(sample_tokens)
 
+    def append_chunked_tokens(self, sample_tokens: List[int]) -> None:
+        """After a chunked-prefill step: every fed prompt advances by its chunk; the prompts completed by it take their
+        first token (the leading entries of `sample_tokens`), the decoding sequences the rest."""
+        i = 0
+        for s, n in zip(self.prefill_bb.seqs_li, self.prefill_chunks):
+            s.num_cached_tokens += n
+            if s.num_cached_tokens == s.input_len:
+                s.output_token_id.append(sample_tokens[i])
+                i += 1
+        if self.decode_in_step and not self.running_bb.is_empty:
+            self.running_bb.append_batch_tokens(torch.tensor(sample_tokens[i:]))
+
     def update(self) -> List[Sequence]:
         """Move freshly prefetched sequences into the decoding bucket, collect finished ones."""
-        if not self.prefill_bb.is_empty:
+        if self.inference_config.max_num_batched_tokens is not None:
+            done = [s for s in self.prefill_bb.seqs_li if s.output_len]         # prompts completed in this step
+            self._index_prefix(self.prefill_bb, done)
+            self.running_bb.merge(self.prefill_bb, [s.request_id for s in done])
+        elif not self.prefill_bb.is_empty:
             self._index_prefix(self.prefill_bb, self.prefill_bb.seqs_li)
             self.running_bb.merge(self.prefill_bb)
         self._index_prefix(self.running_bb, [s for s in self.running_bb.seqs_li if s.check_finish()])
@@ -299,12 +366,14 @@ class RequestHandler(NaiveRequestHandler):
 
     def _index_prefix(self, bucket: BatchBucket, seqs: List[Sequence]) -> None:
         """Prefix caching: index the full blocks of `seqs` whose K/V are written - every position but the last
-        sampled token's (which has none yet, as have rejected speculative tokens)."""
+        sampled token's (which has none yet, as have rejected speculative tokens), or, for a prompt still being
+        prefilled, its first `num_cached_tokens` positions."""
         if not self.inference_config.enable_prefix_caching:
             return
         for s in seqs:
+            written = s.sentence_len - 1 if s.output_len else s.num_cached_tokens
             self.cache_manager.register_prefix_blocks(bucket.block_table_of(s.request_id),
-                                                      s.input_token_id + s.output_token_id, s.sentence_len - 1)
+                                                      s.input_token_id + s.output_token_id, written)
 
     def streamingllm_free_block_tables(self, updated_block_ids: List[int]) -> None:
         self.cache_manager.streamingllm_free_block_tables(updated_block_ids)

@@ -57,6 +57,8 @@ class RPCInferenceEngine(LLMEngine):
         assert self.inference_config.pp_size == 1, "RPC engine: tensor parallelism only"
         if self.inference_config.enable_prefix_caching:
             raise ValueError("the RPC engine does not support enable_prefix_caching")
+        if self.inference_config.max_num_batched_tokens is not None:
+            raise ValueError("the RPC engine does not support max_num_batched_tokens")
 
     # ------------------------------------------------------------------ workers
     def init_workers(self) -> None:

@@ -31,6 +31,32 @@ class PagedKVRuntime:
         self.q_per_seq: int = 1                               # decode: tokens verified per sequence (spec-dec)
         self.max_len_host: int = 0                            # longest sequence of the step (host side, no sync)
         self.cached_prefix = False                            # prompt step where some sequence hit the prefix cache
+        self.chunk_seqs = 0                                   # chunked-prefill step: leading sequences feeding chunks
+        self.chunk_tokens = 0                                 # ... and their rows, which come first
+
+    def set_chunked_step(self, block_tables: torch.Tensor, seq_lens: torch.Tensor, num_cached: List[int],
+                         device) -> torch.Tensor:
+        """Prepare a chunked-prefill step; returns the int64 position of every input token.  The first
+        B_p = len(num_cached) sequences feed a prompt chunk: positions num_cached[b] .. seq_lens[b] - 1, so `seq_lens`
+        counts the cached tokens plus the chunk.  Every other sequence feeds one decode token, at seq_lens[i] - 1.
+        Rows are the chunks, packed by `cu_seqlens` (which covers them only), then the decode rows."""
+        self.block_tables = block_tables.to(device=device, dtype=torch.int32).contiguous()
+        self.seq_lens = seq_lens.to(device=device, dtype=torch.int32).contiguous()
+        self.is_prompt, self.q_per_seq, self.cached_prefix = False, 1, False
+        lens = seq_lens.tolist()
+        self.max_len_host = max(lens)
+        bp = len(num_cached)
+        new = [l - c for l, c in zip(lens[:bp], num_cached)] + [1] * (len(lens) - bp)
+        seq = torch.repeat_interleave(torch.arange(len(lens)), torch.tensor(new))
+        pos = torch.cat([torch.arange(l - n, l) for l, n in zip(lens, new)])
+        cu = torch.zeros(bp + 1, dtype=torch.int32)
+        cu[1:] = torch.cumsum(torch.tensor(new[:bp]), 0)
+        self.cu_seqlens = cu.to(device)
+        self.max_seqlen = max(new[:bp])
+        self.chunk_seqs, self.chunk_tokens = bp, int(cu[-1])
+        self.token_seq = seq.to(device=device, dtype=torch.int32)
+        self.token_pos = pos.to(device=device, dtype=torch.int32)
+        return pos.to(device=device, dtype=torch.int64)
 
     def set_step(self, block_tables: torch.Tensor, seq_lens: torch.Tensor, is_prompt: bool, device,
                  q_per_seq: int = 1, num_cached: Optional[List[int]] = None) -> torch.Tensor:
@@ -44,6 +70,7 @@ class PagedKVRuntime:
         lens = seq_lens.tolist()
         self.max_len_host = max(lens) if lens else 0
         self.cached_prefix = False
+        self.chunk_seqs = 0
         if is_prompt:
             cached = num_cached if num_cached is not None else [0] * len(lens)
             self.cached_prefix = any(c > 0 for c in cached)
@@ -66,6 +93,8 @@ class PagedKVRuntime:
                alibi_slopes: Optional[torch.Tensor] = None, sliding_window: Optional[int] = None) -> torch.Tensor:
         kc, vc = self.k_caches[layer_idx], self.v_caches[layer_idx]
         iops.kv_cache_write(k, v, kc, vc, self.block_tables, self.token_seq, self.token_pos)
+        if self.chunk_seqs:
+            return self._attend_chunked(q, kc, vc, scale, alibi_slopes, sliding_window)
         if self.is_prompt and self.cached_prefix:
             # prefix-cache hit: the new rows attend over the cached prefix and their own K/V, all in the paged cache
             window = sliding_window if sliding_window is not None and self.max_len_host > sliding_window else None
@@ -74,6 +103,20 @@ class PagedKVRuntime:
         if sliding_window is not None and self.max_len_host > sliding_window:
             return self._attend_windowed(q, k, v, kc, vc, scale, alibi_slopes, sliding_window)
         return self._attend_full(q, k, v, kc, vc, scale, alibi_slopes)
+
+    def _attend_chunked(self, q, kc, vc, scale, alibi_slopes, sliding_window) -> torch.Tensor:
+        """Chunked-prefill step: the chunk rows attend through the paged prefill (each chunk follows its prompt's
+        earlier chunks, already in the cache), the decode rows through the split-KV paged decode.  The boundaries
+        are host values, so nothing syncs."""
+        bp, tp = self.chunk_seqs, self.chunk_tokens
+        window = sliding_window if sliding_window is not None and self.max_len_host > sliding_window else None
+        out = iops.paged_prefill_attention(q[:tp], kc, vc, self.block_tables[:bp], self.cu_seqlens,
+                                           self.seq_lens[:bp], scale, alibi_slopes=alibi_slopes, window=window)
+        if tp == q.shape[0]:
+            return out
+        dec = iops.paged_decode_attention(q[tp:], kc, vc, self.block_tables[bp:], self.seq_lens[bp:], scale,
+                                          alibi_slopes=alibi_slopes, window=window)
+        return torch.cat([out, dec])
 
     def _native_prefill(self, q, k, v, scale, window: int, alibi_slopes) -> Optional[torch.Tensor]:
         """Sliding-window / ALiBi prefill inside the wgmma flash kernel (packed batch, device-resident boundaries);

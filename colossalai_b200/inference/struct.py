@@ -46,8 +46,9 @@ class Sequence:
     def __post_init__(self) -> None:
         self.output_token_id: List[int] = []
         self.status = RequestStatus.WAITING
-        # prompt tokens whose K/V came from the prefix cache at admission (a whole number of blocks); the prefill
-        # computes and writes only the positions from here on
+        # prompt tokens whose K/V the cache holds while the prompt is prefilled: the prefix-cache hit at admission (a
+        # whole number of blocks), advanced by each chunk under chunked prefill.  The prefill computes and writes only
+        # the positions from here on
         self.num_cached_tokens = 0
 
     @property
